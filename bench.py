@@ -1,14 +1,14 @@
-"""Headline benchmark: ResNet-50 training images/sec on N B200s (BASELINE.json metric / config).
+"""Headline benchmark: ResNet-50 training images/sec on N H100s (BASELINE.json metric / config).
 
     python bench.py --gpus 1 --steps 20 --warmup 5
     python -m torch.distributed.run --nnodes=1 --nproc-per-node 8 --master-addr 127.0.0.1 --master-port P bench.py --gpus 8 ...
-    python bench.py --impl reference ...        (the unmodified reference scripts from baseline/_ref, stock code path)
+    python bench.py --impl reference ...        (the unmodified reference scripts from oracle/_ref, stock code path)
 
 Own arm: the public training path of this repo (driver.Strategy.build -> DistributedDataParallel + FusedSGD, the
 DataPrefetcher, the MetricPipeline) - the same objects `distributed.py` uses.
   value       device-timed (CUDA events, max over ranks) images/s of K full training steps
               (forward + loss + metric kernel + backward with fused all-reduce + optimizer), inputs already on the
-              device (4 distinct 256-image bf16 NHWC batches = 154 MB > the 126 MB L2; activations are GBs).
+              device (4 distinct 256-image bf16 NHWC batches = 154 MB > the 50 MB L2; activations are GBs).
   e2e.value   the same loop fed from PINNED HOST memory through the prefetcher (H2D of every batch inside the timed
               region) with the step's reduced loss/accuracy copied back to the host every step.
 Synthetic data, random-init weights, weak scaling (256 images per GPU).
@@ -49,6 +49,8 @@ def parse():
     p.add_argument("--no-cuda-graph", action="store_true")
     p.add_argument("--entry", default="distributed", choices=["distributed", "apex_distributed", "horovod_distributed", "dataparallel"])
     p.add_argument("--opt-level", default="O2")
+    p.add_argument("--dump-outputs", metavar="DIR", default=None,
+                   help="write the last timed step's results to DIR/<name>.npy (rank 0) to compare two builds")
     return p.parse_args()
 
 
@@ -142,6 +144,22 @@ class ClockSampler:
                 "reasons": sorted(self.reasons), "samples": len(self.sm), "source": self.mode}
 
 
+DUMP_SAMPLE = 1 << 22      # state entries kept by --dump-outputs: 16 MB of float32
+
+
+def dump_outputs(directory: str, model, metrics) -> None:
+    """What the timed step hands its caller, after the last timed step: the reduced loss / top-1 / top-5 of that step
+    (``metrics.npy``, float64) and the trained model state - every floating-point entry of ``state_dict()`` (weights
+    and BatchNorm running statistics) flattened in order, of which the ``DUMP_SAMPLE`` positions drawn with a fixed
+    seed are written in ascending order (``state_sample.npy``, float32)."""
+    import numpy as np
+    os.makedirs(directory, exist_ok=True)
+    np.save(os.path.join(directory, "metrics.npy"), np.asarray(metrics.last, dtype=np.float64))
+    flat = torch.cat([t.detach().reshape(-1).float() for t in model.state_dict().values() if t.is_floating_point()])
+    idx = np.sort(np.random.default_rng(0).choice(flat.numel(), size=min(flat.numel(), DUMP_SAMPLE), replace=False))
+    np.save(os.path.join(directory, "state_sample.npy"), flat[torch.from_numpy(idx).to(flat.device)].cpu().numpy())
+
+
 def dist_env():
     if "RANK" in os.environ and "WORLD_SIZE" in os.environ:
         return int(os.environ["RANK"]), int(os.environ.get("LOCAL_RANK", 0)), int(os.environ["WORLD_SIZE"])
@@ -190,10 +208,15 @@ def run_own(a):
     st = driver.STRATEGIES[a.entry]()
     if world > 1 or a.entry == "horovod_distributed":
         st.init_process_group(args, local_rank, world)
+    torch.manual_seed(0)                    # the same weights on every run: --dump-outputs compares builds
     model = create_model(args.arch, num_classes=args.num_classes, fused_bn=args.fused_bn)
     model, optimizer = st.build(model, args, device, local_rank)
     criterion = torch.nn.CrossEntropyLoss().to(device)
-    torch.backends.cudnn.benchmark = True
+    # cuDNN as distributed.py runs it (algorithms picked by timing them).  --dump-outputs needs the same results on every
+    # run instead: deterministic algorithms chosen by heuristics (a timed choice can differ from run to run, and so can
+    # its rounding).  The JSON line records which of the two the timed steps used.
+    torch.backends.cudnn.benchmark = not a.dump_outputs
+    torch.backends.cudnn.deterministic = bool(a.dump_outputs)
     B = a.batch_per_gpu * (a.gpus if dp else 1)
     W, K = a.warmup, a.steps
     losses, top1, top5 = AverageMeter("Loss"), AverageMeter("Acc@1"), AverageMeter("Acc@5")
@@ -234,6 +257,8 @@ def run_own(a):
     launches = _ext.launches - n0
     clocks = sampler.stop() if rank == 0 else None
     metrics.drain()
+    if a.dump_outputs and rank == 0:
+        dump_outputs(a.dump_outputs, model, metrics)
     ms = max_over_ranks(ev0.elapsed_time(ev1), device)
     value = B * world * K / (ms / 1e3)
     # PTD_PYPROFILE=<file>: cProfile of 5 extra steps (host-side cost of a step; outside the timed region)
@@ -304,6 +329,7 @@ def run_own(a):
                        "l2_policy": "inputs larger than L2 (4 x 38.5 MB bf16 batches + GBs of activations per step)",
                        "bucket_cap_mb": args.bucket_cap_mb, "overlap_optimizer": bool(getattr(optimizer, "_overlap", False)),
                        "bucket_view": bool(getattr(args, "bucket_view", False)),
+                       "cudnn": "deterministic" if a.dump_outputs else "benchmark",
                        "opt_in": {k: os.environ[k] for k in ("PTD_SPLIT_RESGRAD", "PTD_STEM_GEMM", "PTD_FUSED_CONV1X1", "PTD_MAX_CTAS",
                                                              "PTD_NVLS", "PTD_BENCH_ARGS", "PTD_DEFERRED_BCAST", "PTD_METRICS_SIDE",
                                                              "PTD_ONESHOT_MAX_BYTES", "PTD_HVD_STATIC") if k in os.environ}},
@@ -330,7 +356,7 @@ def published_baseline():
 
 # ====================================================================== reference arm
 def run_reference(a):
-    from baseline.run_reference import run
+    from oracle.run_reference import run
     run(a, METRIC, ClockSampler, published_baseline)
 
 

@@ -1,7 +1,7 @@
-"""Builds and loads the native sm_100a extension (``pytorch_distributed_b200/_C*.so``, in-tree).
+"""Builds and loads the native sm_90a extension (``pytorch_distributed_b200/_C*.so``, in-tree).
 
 * ``build()`` compiles every source under ``csrc/`` with
-  ``-gencode arch=compute_100a,code=sm_100a -lineinfo`` (nvcc cross-compiles without a GPU) and drops the shared
+  ``-gencode arch=compute_90a,code=sm_90a -lineinfo`` (nvcc cross-compiles without a GPU) and drops the shared
   object next to this file, so it travels with the source tree.  A content hash of the sources is stored beside it;
   a stale or missing build is redone on import when a compiler is available.
 * ``lib()`` returns the module or raises.  On a CUDA machine a missing extension is a hard error - there is no
@@ -26,7 +26,7 @@ _lock = threading.Lock()
 _mod = None
 _err = None
 
-CUDA_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "--use_fast_math", "-std=c++17",
+CUDA_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "--use_fast_math", "-std=c++17",
               "--expt-relaxed-constexpr", "-Xptxas", "-v"]
 
 
@@ -49,7 +49,7 @@ def is_built() -> bool:
 
 
 def build(verbose: bool = False, force: bool = False) -> str:
-    """Compile the extension in-tree for sm_100a. Returns the path of the shared object."""
+    """Compile the extension in-tree for sm_90a. Returns the path of the shared object."""
     with _lock:
         if is_built() and not force:
             return _SO

@@ -1,6 +1,6 @@
 """Builds and loads the host-only native module (``pytorch_distributed_b200/_L.so``): the C++ shard loader.
 
-Kept apart from ``_C`` (the sm_100a extension) on purpose: it has no CUDA or libtorch dependency, compiles with plain
+Kept apart from ``_C`` (the sm_90a extension) on purpose: it has no CUDA or libtorch dependency, compiles with plain
 ``g++`` in a few seconds, and is usable on machines without nvcc.  Same in-tree + content-hash scheme as ``_ext``.
 """
 from __future__ import annotations

@@ -20,7 +20,7 @@ def model_names():
 
 
 def build_parser(entry: str = "distributed") -> argparse.ArgumentParser:
-    p = argparse.ArgumentParser(description="B200-native ImageNet training (%s)" % entry)
+    p = argparse.ArgumentParser(description="H100-native ImageNet training (%s)" % entry)
     p.add_argument("--data", metavar="DIR", default=os.environ.get("IMAGENET_DIR", ""),
                    help="path to dataset (DIR/train, DIR/val ImageFolder trees); "
                         "empty or --synthetic => synthetic ImageNet-shaped data")
@@ -61,7 +61,7 @@ def build_parser(entry: str = "distributed") -> argparse.ArgumentParser:
         p.add_argument("--compression", default="fp16", choices=["none", "fp16", "bf16"],
                        help="wire compression for the DistributedOptimizer (reference: fp16)")
 
-    # ---- additive, B200-native knobs (all have reference-compatible defaults) ----
+    # ---- additive, H100-native knobs (all have reference-compatible defaults) ----
     x = p.add_argument_group("b200")
     x.add_argument("--synthetic", action="store_true", help="force synthetic ImageNet-shaped data")
     x.add_argument("--synthetic-size", default=None, type=int, metavar="N",
@@ -72,7 +72,7 @@ def build_parser(entry: str = "distributed") -> argparse.ArgumentParser:
     x.add_argument("--image-size", default=224, type=int)
     x.add_argument("--num-classes", default=1000, type=int)
     x.add_argument("--comm", default="auto", choices=["auto", "fused", "nccl", "gloo"],
-                   help="gradient data plane: fused = sm_100a peer-memory kernels, nccl/gloo = library all-reduce")
+                   help="gradient data plane: fused = sm_90a peer-memory kernels, nccl/gloo = library all-reduce")
     x.add_argument("--wire-dtype", default="bf16", choices=["bf16", "fp16", "fp32"],
                    help="gradient wire format of the fused all-reduce")
     x.add_argument("--bucket-cap-mb", default=8.0, type=float,

@@ -30,7 +30,7 @@ at::Tensor arena_view(const std::shared_ptr<SymmArena>& a, int64_t rank, int64_t
 }  // namespace
 
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
-  m.doc() = "pytorch_distributed_b200 native runtime (sm_100a)";
+  m.doc() = "pytorch_distributed_b200 native runtime (sm_90a)";
   m.attr("MAX_WORLD") = kMaxWorld;
   m.attr("MAX_BLOCKS") = kMaxBlocks;
   m.attr("MAX_CHANNELS") = kMaxChannels;

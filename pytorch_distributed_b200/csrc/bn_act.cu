@@ -1,8 +1,8 @@
-// Fused NHWC BatchNorm (+ residual add) (+ ReLU), forward and backward, for sm_100a.
+// Fused NHWC BatchNorm (+ residual add) (+ ReLU), forward and backward, for sm_90a.
 //
 // The reference reaches cuDNN BN + ATen add + ATen ReLU through torchvision's ResNet
-// (/root/reference/distributed.py:136-139,250).  On B200 a bf16 ResNet-50 step is bound by exactly those
-// memory passes (45% of the step in the first profile, profiles/step_breakdown_r1.md), so they are fused here:
+// (reference distributed.py:136-139,250).  A bf16 ResNet-50 step is bound by exactly those memory passes, so they
+// are fused here:
 //   forward : stats pass (1 read)  + apply pass  (x [+res] -> y, 1-bit ReLU mask)             eager: 3-5 R, 2-3 W
 //   backward: reduce pass (dy,x,mask) + apply pass (dy,x,mask -> dx [,dres])                   eager: 6 R, 2-3 W
 // The ReLU decision is kept as ONE BIT per element (a byte per thread-vector of 8 channels), so the backward never
@@ -62,9 +62,10 @@ __device__ __forceinline__ void st_w(void* p, int dt, int i, float v) {
   }
 }
 
-// Combine the per-thread partial sums (a[8], b[8] for channel group `cg`) of a CTA into gsum[0:C] / gsum[C:2C].
+// Combine the per-thread partial sums (a[8], b[8] for channel group `cg`) of a CTA into this CTA's row of the partials,
+// part[blockIdx.x][0:C] / [C:2C]; combine_partials() then adds the rows in a fixed order.
 // Caller loops over channel-group chunks; `sm` holds [slots][2 * tpr * 8] floats.
-__device__ __forceinline__ void cta_combine(const RowMap& m, int cg_base, float (&a)[8], float (&b)[8], float* sm, float* gsum, int C) {
+__device__ __forceinline__ void cta_combine(const RowMap& m, int cg_base, float (&a)[8], float (&b)[8], float* sm, float* part, int C) {
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int width = m.tpr * 8;        // channels covered per pass
   int slots, slot;
@@ -95,13 +96,43 @@ __device__ __forceinline__ void cta_combine(const RowMap& m, int cg_base, float 
     float s = 0.f;
     for (int r = 0; r < slots; ++r) s += sm[(size_t)r * 2 * width + i];
     const int half = i >= width, c = cg_base * 8 + (i - half * width);
-    if (c < C) atomicAdd(&gsum[half * C + c], s);
+    if (c < C) part[(size_t)blockIdx.x * 2 * C + half * C + c] = s;
   }
+}
+
+// gsum[i] += sum over b of part[b * n + i], always in the same order (b ascending within each of 32 slices, then the 32
+// slice sums in order).  Float atomics across CTAs would make every BatchNorm statistic - and everything trained from
+// it - depend on CTA scheduling; this way a step computes the same bits on every run.
+__global__ void __launch_bounds__(1024) combine_partials_kernel(const float* __restrict__ part, int nblocks, int n,
+                                                                float* __restrict__ gsum) {
+  __shared__ float sm[32][33];
+  const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
+  const int i = blockIdx.x * 32 + tx;
+  float s = 0.f;
+  if (i < n)
+    for (int b = ty; b < nblocks; b += 32) s += part[(size_t)b * n + i];
+  sm[ty][tx] = s;
+  __syncthreads();
+  if (ty == 0 && i < n) {
+    float t = 0.f;
+    for (int k = 0; k < 32; ++k) t += sm[k][tx];
+    gsum[i] += t;
+  }
+}
+
+void combine_partials(const float* part, int nblocks, int n, float* gsum, cudaStream_t st) {
+  combine_partials_kernel<<<(n + 31) / 32, 1024, 0, st>>>(part, nblocks, n, gsum);
+  C10_CUDA_KERNEL_LAUNCH_CHECK();
+}
+
+// per-CTA partial sums [grid][2C] of one reduction pass
+static at::Tensor partials(const at::Tensor& x, int grid, int C) {
+  return at::empty({grid, 2 * C}, x.options().dtype(at::kFloat).memory_format(at::MemoryFormat::Contiguous));
 }
 
 // ------------------------------------------------------------------ forward: statistics
 template <typename T>
-__global__ void __launch_bounds__(kBnThreads) bn_stats_kernel(const T* __restrict__ x, float* __restrict__ gsum, int64_t M, int C,
+__global__ void __launch_bounds__(kBnThreads) bn_stats_kernel(const T* __restrict__ x, float* __restrict__ part, int64_t M, int C,
                                                               int rows_per_block) {
   extern __shared__ float sm[];
   const RowMap m = row_map(C);
@@ -130,7 +161,7 @@ __global__ void __launch_bounds__(kBnThreads) bn_stats_kernel(const T* __restric
         for (int k = 0; k < 8; ++k) { s[k] += f[k]; q[k] += f[k] * f[k]; }
       }
     }
-    cta_combine(m, cgb, s, q, sm, gsum, C);
+    cta_combine(m, cgb, s, q, sm, part, C);
   }
 }
 
@@ -220,7 +251,7 @@ __global__ void __launch_bounds__(kBnThreads) bn_apply_kernel(const T* __restric
 template <typename T, bool RELU>
 __global__ void __launch_bounds__(kBnThreads) bn_bwd_reduce_kernel(const T* __restrict__ dy, const uint8_t* __restrict__ mask,
                                                                    const T* __restrict__ x, const float* __restrict__ saved,
-                                                                   float* __restrict__ gsum, int64_t M, int C, int rows_per_block) {
+                                                                   float* __restrict__ part, int64_t M, int C, int rows_per_block) {
   extern __shared__ float sm[];
   const RowMap m = row_map(C);
   const int64_t r0 = (int64_t)blockIdx.x * rows_per_block, r1 = min(M, r0 + (int64_t)rows_per_block);
@@ -272,7 +303,7 @@ __global__ void __launch_bounds__(kBnThreads) bn_bwd_reduce_kernel(const T* __re
 #pragma unroll
       for (int k = 0; k < 8; ++k) q[k] *= saved[C + cg * 8 + k];   // x invstd once per CTA, not per element
     }
-    cta_combine(m, cgb, s, q, sm, gsum, C);
+    cta_combine(m, cgb, s, q, sm, part, C);
   }
 }
 
@@ -422,8 +453,10 @@ static void fwd_impl(const at::Tensor& x, const at::Tensor* res, at::Tensor& y, 
   if (training && !stats_ready) {     // stats_ready: the producing GEMM already reduced sum / sum-of-squares (gemm_bnstats.cu)
     int rpb;
     const int grid = reduce_grid(g, &rpb, resident_ctas(bn_stats_kernel<T>, g.smem));
-    bn_stats_kernel<T><<<grid, kBnThreads, g.smem, st>>>(xp, wk, g.M, g.C, rpb);
+    at::Tensor part = partials(x, grid, g.C);
+    bn_stats_kernel<T><<<grid, kBnThreads, g.smem, st>>>(xp, part.data_ptr<float>(), g.M, g.C, rpb);
     C10_CUDA_KERNEL_LAUNCH_CHECK();
+    combine_partials(part.data_ptr<float>(), grid, 2 * g.C, wk, st);
   }
   const int grid = apply_grid(g);
   float* rmp = rm.defined() ? rm.data_ptr<float>() : nullptr;
@@ -490,9 +523,12 @@ static void bwd_impl(const at::Tensor& dy, const at::Tensor& mask, const at::Ten
   int rpb;
   const int rgrid = reduce_grid(g, &rpb, relu ? resident_ctas(bn_bwd_reduce_kernel<T, true>, g.smem)
                                              : resident_ctas(bn_bwd_reduce_kernel<T, false>, g.smem));
-  if (relu) bn_bwd_reduce_kernel<T, true><<<rgrid, kBnThreads, g.smem, st>>>(dyp, mk, xp, sv, wk, g.M, g.C, rpb);
-  else      bn_bwd_reduce_kernel<T, false><<<rgrid, kBnThreads, g.smem, st>>>(dyp, mk, xp, sv, wk, g.M, g.C, rpb);
+  at::Tensor part = partials(x, rgrid, g.C);
+  float* pp = part.data_ptr<float>();
+  if (relu) bn_bwd_reduce_kernel<T, true><<<rgrid, kBnThreads, g.smem, st>>>(dyp, mk, xp, sv, pp, g.M, g.C, rpb);
+  else      bn_bwd_reduce_kernel<T, false><<<rgrid, kBnThreads, g.smem, st>>>(dyp, mk, xp, sv, pp, g.M, g.C, rpb);
   C10_CUDA_KERNEL_LAUNCH_CHECK();
+  combine_partials(pp, rgrid, 2 * g.C, wk, st);
   const int grid = apply_grid(g);
   T* dxp = reinterpret_cast<T*>(dx.data_ptr());
   T* drp = write_res ? reinterpret_cast<T*>(dres.data_ptr()) : nullptr;
@@ -545,7 +581,7 @@ template <typename T, bool RELU>
 __global__ void __launch_bounds__(kBnThreads) bn_bwd_reduce_sum_kernel(const T* __restrict__ dya, const T* __restrict__ dyb,
                                                                        const uint8_t* __restrict__ mask, const T* __restrict__ x,
                                                                        const float* __restrict__ saved, T* __restrict__ gout,
-                                                                       float* __restrict__ gsum, int64_t M, int C, int rows_per_block) {
+                                                                       float* __restrict__ part, int64_t M, int C, int rows_per_block) {
   extern __shared__ float sm[];
   const RowMap m = row_map(C);
   const int64_t r0 = (int64_t)blockIdx.x * rows_per_block, r1 = min(M, r0 + (int64_t)rows_per_block);
@@ -604,7 +640,7 @@ __global__ void __launch_bounds__(kBnThreads) bn_bwd_reduce_sum_kernel(const T* 
 #pragma unroll
       for (int k = 0; k < 8; ++k) q[k] *= saved[C + cg * 8 + k];
     }
-    cta_combine(m, cgb, s, q, sm, gsum, C);
+    cta_combine(m, cgb, s, q, sm, part, C);
   }
 }
 
@@ -623,9 +659,12 @@ static void bwd2_impl(const at::Tensor& dya, const at::Tensor& dyb, const at::Te
   int rpb;
   const int rgrid = reduce_grid(g, &rpb, relu ? resident_ctas(bn_bwd_reduce_sum_kernel<T, true>, g.smem)
                                              : resident_ctas(bn_bwd_reduce_sum_kernel<T, false>, g.smem));
-  if (relu) bn_bwd_reduce_sum_kernel<T, true><<<rgrid, kBnThreads, g.smem, st>>>(ap, bp, mk, xp, sv, gp, wk, g.M, g.C, rpb);
-  else      bn_bwd_reduce_sum_kernel<T, false><<<rgrid, kBnThreads, g.smem, st>>>(ap, bp, mk, xp, sv, gp, wk, g.M, g.C, rpb);
+  at::Tensor part = partials(x, rgrid, g.C);
+  float* pp = part.data_ptr<float>();
+  if (relu) bn_bwd_reduce_sum_kernel<T, true><<<rgrid, kBnThreads, g.smem, st>>>(ap, bp, mk, xp, sv, gp, pp, g.M, g.C, rpb);
+  else      bn_bwd_reduce_sum_kernel<T, false><<<rgrid, kBnThreads, g.smem, st>>>(ap, bp, mk, xp, sv, gp, pp, g.M, g.C, rpb);
   C10_CUDA_KERNEL_LAUNCH_CHECK();
+  combine_partials(pp, rgrid, 2 * g.C, wk, st);
   // second pass: g already carries the mask, and it IS the residual gradient -> the plain (no ReLU, no dres) apply variant
   bn_bwd_apply_kernel<T, false, false><<<apply_grid(g), kBnThreads, 0, st>>>(gp, nullptr, xp, sv, wk, w.data_ptr(), wdtype(w),
                                                                            reinterpret_cast<T*>(dx.data_ptr()), nullptr, dw.data_ptr(),
@@ -672,7 +711,7 @@ std::vector<at::Tensor> bn_act_backward2(const at::Tensor& dy_a_in, const at::Te
 //
 // torchvision's stem (/root/reference/distributed.py:136-139 -> resnet.conv1/bn1/relu/maxpool) writes the full
 // 112x112 activation, re-reads it for the pool, and in backward runs ATen's max_pool_backward_nhwc with int64 indices
-// (1.7 ms / step on B200, see profiles/).  Here the normalised activation never touches HBM:
+// (int64 index traffic).  Here the normalised activation never touches HBM:
 //   forward : one pass over the conv output: BN -> ReLU -> 3x3 max -> pooled output + a 4-bit arg-max code per element
 //             (code 15 = "all candidates <= 0": the ReLU killed the gradient)
 //   backward: two passes over the INPUT domain; each input position gathers the (at most 4) pooled gradients whose
@@ -899,7 +938,7 @@ __device__ __forceinline__ void stem_quad_dz(const T* __restrict__ dp, const uin
 template <typename T>
 __global__ void __launch_bounds__(kBnThreads, 4) stem_bwd_reduce_kernel(const T* __restrict__ dp, const uint2* __restrict__ code,
                                                                      const T* __restrict__ x, const float* __restrict__ saved,
-                                                                     float* __restrict__ gsum, int64_t M, int C, PoolGeom g,
+                                                                     float* __restrict__ part, int64_t M, int C, PoolGeom g,
                                                                      int rows_per_block) {
   extern __shared__ float sm[];
   const RowMap m = row_map(C);                       // tpr == cgs (host guarantees cgs divides the CTA size)
@@ -944,7 +983,7 @@ __global__ void __launch_bounds__(kBnThreads, 4) stem_bwd_reduce_kernel(const T*
   }
 #pragma unroll
   for (int k = 0; k < 8; ++k) q[k] *= saved[C + cg * 8 + k];
-  cta_combine(m, 0, s, q, sm, gsum, C);
+  cta_combine(m, 0, s, q, sm, part, C);
 }
 
 template <typename T>
@@ -1017,8 +1056,10 @@ static void stem_fwd_impl(const at::Tensor& x, at::Tensor& y, at::Tensor& code, 
   if (training && !stats_ready) {      // stats_ready: the producing GEMM already reduced sum / sum-of-squares into `work`
     int rpb;
     const int grid = reduce_grid(g, &rpb, resident_ctas(bn_stats_kernel<T>, g.smem));
-    bn_stats_kernel<T><<<grid, kBnThreads, g.smem, st>>>(xp, wk, g.M, g.C, rpb);
+    at::Tensor part = partials(x, grid, g.C);
+    bn_stats_kernel<T><<<grid, kBnThreads, g.smem, st>>>(xp, part.data_ptr<float>(), g.M, g.C, rpb);
     C10_CUDA_KERNEL_LAUNCH_CHECK();
+    combine_partials(part.data_ptr<float>(), grid, 2 * g.C, wk, st);
   }
   const int cgs = g.C / 8;
   const int64_t total = x.size(0) * pg.OH * pg.OW;
@@ -1086,8 +1127,10 @@ static void stem_bwd_impl(const at::Tensor& dp, const at::Tensor& code, const at
   const int nrows = (int)(x.size(0) * ((pg.H + 1) / 2));               // quad rows
   const int rpb = std::max(1, std::min(4, nrows / (g.sms * 8)));       // quad rows per CTA
   const int grid = (nrows + rpb - 1) / rpb;
-  stem_bwd_reduce_kernel<T><<<grid, kBnThreads, g.smem, st>>>(dpp, cp, xp, saved.data_ptr<float>(), work.data_ptr<float>(), g.M, g.C, pg, rpb);
+  at::Tensor part = partials(x, grid, g.C);
+  stem_bwd_reduce_kernel<T><<<grid, kBnThreads, g.smem, st>>>(dpp, cp, xp, saved.data_ptr<float>(), part.data_ptr<float>(), g.M, g.C, pg, rpb);
   C10_CUDA_KERNEL_LAUNCH_CHECK();
+  combine_partials(part.data_ptr<float>(), grid, 2 * g.C, work.data_ptr<float>(), st);
   stem_bwd_apply_kernel<T><<<grid, kBnThreads, 0, st>>>(dpp, cp, xp, saved.data_ptr<float>(), work.data_ptr<float>(), w.data_ptr(), wdtype(w),
                                                        reinterpret_cast<T*>(dx.data_ptr()), dw.data_ptr(), db.data_ptr(), g.M, g.C, pg, rpb);
   C10_CUDA_KERNEL_LAUNCH_CHECK();

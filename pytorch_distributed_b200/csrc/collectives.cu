@@ -1,4 +1,4 @@
-// Fused multi-tensor collectives over NVLink 5 / NVSwitch peer memory (sm_100a).
+// Fused multi-tensor collectives over NVLink / NVSwitch peer memory (sm_90a).
 //
 //   K1  fused_allreduce   : (cast+scale+pack) -> barrier -> reduce-scatter+all-gather -> barrier -> (unpack)
 //                           one kernel per gradient bucket, launched from the backward hooks.

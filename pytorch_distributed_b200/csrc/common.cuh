@@ -1,4 +1,4 @@
-// Device-side building blocks shared by every sm_100a kernel in this extension:
+// Device-side building blocks shared by every sm_90a kernel in this extension:
 //  * 16-byte vector load/store with explicit cache policy
 //  * NVLS multimem.ld_reduce / multimem.st wrappers (in-switch reduction / multicast over NVSwitch)
 //  * system-scope signal flags (monotonic sequence numbers, no reset) + block barrier across GPUs

@@ -1,22 +1,23 @@
-// 1x1 convolution (NHWC) as a tcgen05 GEMM with the BatchNorm statistics fused into the epilogue (sm_100a).
+// 1x1 convolution (NHWC) as a wgmma GEMM with the BatchNorm statistics fused into the epilogue (sm_90a).
 //
 //   C[M, N] (bf16) = A[M, K] (bf16 activations, K = C_in contiguous) x B[N, K]^T (bf16 weights [C_out, C_in])
-//   gsum[0:N]  += sum_m C[m, n]          gsum[N:2N] += sum_m C[m, n]^2          (fp32, from the fp32 accumulators)
+//   gsum[0:N]  += sum_m C[m, n]          gsum[N:2N] += sum_m C[m, n]^2          (fp32, over the stored bf16 values)
 //
-// In a ResNet-50 step the 1x1 convolutions are HBM-bound (profiles/conv1x1_probe: cuDNN == cuBLAS == ~6 TB/s), so the
-// only way to make them cheaper is to do more per byte: the per-channel sum / sum-of-squares that BatchNorm needs are
-// reduced here from the accumulators while they sit in tensor memory, which removes BN's separate statistics pass
-// (one full re-read of the conv output).  Reference call site: every conv1x1 -> bn pair of torchvision's Bottleneck
-// reached through /root/reference/distributed.py:136-139.
+// In a ResNet-50 step the 1x1 convolutions are HBM-bound, so the only way to make them cheaper is to do more per byte:
+// the per-channel sum / sum-of-squares that BatchNorm needs are reduced here from the output tile while it sits in
+// shared memory on its way out, which removes BN's separate statistics pass (one full re-read of the conv output).
+// Call site: every conv1x1 -> bn pair of the Bottleneck blocks (models/resnet.py, ops/conv_bn.py) and the stem GEMM.
 //
-// Blackwell structure (one 128 x BLOCK_N output tile per CTA, up to two CTAs per SM so that one CTA's epilogue
-// overlaps the other's loads):
-//   warp 0      TMA producer : cp.async.bulk.tensor.2d (128B-swizzled 128x64 A tile, BLOCK_Nx64 B tile) -> smem ring,
-//                              completion on an mbarrier (expect_tx)
-//   warp 1      MMA issuer   : allocates BLOCK_N TMEM columns, one elected thread issues tcgen05.mma.cta_group::1.kind::f16
-//                              (M=128, N=BLOCK_N, K=16) x4 per stage from smem descriptors, tcgen05.commit frees the stage
-//   warps 2..5  epilogue     : tcgen05.ld 32 lanes x 32 columns per warp (each warp owns its TMEM lane quadrant),
-//                              butterfly transpose-reduce across lanes for the column sums, bf16 pack, 64-byte row stores
+// Hopper structure: persistent CTAs, one per SM, each with a FIXED n-tile (so its per-channel partial sums stay in
+// registers for the CTA's lifetime and reach global memory once) and m-tiles strided by the number of CTAs per n-tile;
+// CTAs with adjacent ids share the same m-tile sequence, so an A tile is fetched from HBM once and hit in L2 by the
+// other n-tiles.
+//   warp 8        TMA producer : cp.async.bulk.tensor.2d (128B-swizzled 128x64 A tile, BLOCK_Nx64 B tile) -> smem ring,
+//                                completion on an mbarrier (expect_tx); runs ahead across tile boundaries
+//   warpgroups 0,1 consumers   : warpgroup c owns rows [64c, 64c+64) of the 128-row tile; wgmma.mma_async m64nXk16
+//                                (bf16 x bf16 -> fp32 registers) straight from the swizzled smem stages; epilogue packs
+//                                bf16 into a 128B-swizzled staging tile, one TMA store per 64x64 box (clipped at the M
+//                                tail by the tensor map), column owners reduce the statistics from the staged values.
 #include <ATen/cuda/CUDAContext.h>
 #include <c10/cuda/CUDAGuard.h>
 #include <cuda.h>
@@ -27,10 +28,19 @@
 
 namespace ptd {
 
-constexpr int kGemmThreads = 192;
 constexpr int kBlockM = 128;
-constexpr int kBlockK = 64;   // 64 bf16 = one 128-byte swizzle row
-constexpr int kStages = 2;
+constexpr int kBlockK = 64;          // 64 bf16 = one 128-byte swizzle row
+constexpr int kConsumerThreads = 256;
+constexpr int kGemmThreads = kConsumerThreads + 32;
+
+template <int BLOCK_N> struct GemmCfg {
+  static constexpr int kStages = BLOCK_N == 256 ? 3 : 4;
+  static constexpr int kABytes = kBlockM * kBlockK * 2;
+  static constexpr int kBBytes = BLOCK_N * kBlockK * 2;
+  static constexpr int kCBytes = kBlockM * BLOCK_N * 2;               // bf16 output staging, [BLOCK_N / 64] 64-column boxes
+  static constexpr int kStatFloats = 2 * 4 * 128;                     // [2 warpgroups][4 sums][128 threads]
+  static constexpr int kSmem = 1024 + kStages * (kABytes + kBBytes) + kCBytes + kStatFloats * 4 + 2 * kStages * 8;
+};
 
 // ------------------------------------------------------------------ PTX wrappers
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -40,6 +50,9 @@ __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
 }
 __device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
+  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   const uint32_t addr = smem_u32(bar);
@@ -54,211 +67,67 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* m
   asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
                ::"r"(smem_u32(smem_dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1) : "memory");
 }
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred;
-  asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(pred));
-  return pred != 0;
+__device__ __forceinline__ void named_barrier(int id, int threads) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
 }
-// K-major, 128-byte swizzle: 8-row groups are 1024 bytes apart (SBO), LBO unused (=1), descriptor version 1 (Blackwell)
-__device__ __forceinline__ uint64_t umma_desc(const void* smem_tile) {
+
+// wgmma shared-memory matrix descriptor: K-major, 128-byte swizzle, 8-row groups 1024 bytes apart (SBO), LBO unused (=1).
+// The tile is 1024-byte aligned; +2 in the (>>4) start-address field advances K by 16 bf16 (32 bytes).
+__device__ __forceinline__ uint64_t gmma_desc(const void* smem_tile) {
   const uint64_t addr = (uint64_t)(smem_u32(smem_tile) >> 4) & 0x3FFFull;
-  return addr | (1ull << 16) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 46) | (2ull << 61);
-}
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, bool accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc),
-      "r"((uint32_t)accumulate) : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-        "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]),
-        "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-        "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+  return addr | (1ull << 16) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 62);
 }
 
-// lane L ends up with sum over the 32 lanes of v[L] (butterfly transpose-reduce: 31 shuffles instead of 160)
-__device__ __forceinline__ float column_reduce(float (&v)[32], int lane) {
+#define PTD_F8(i) "+f"(d[i]), "+f"(d[i + 1]), "+f"(d[i + 2]), "+f"(d[i + 3]), "+f"(d[i + 4]), "+f"(d[i + 5]), "+f"(d[i + 6]), "+f"(d[i + 7])
+
+// D[64 x 64] (+)= A[64 x 16] * B[64 x 16]^T, fp32 accumulators in d[32]
+__device__ __forceinline__ void wgmma_n64(float* d, uint64_t adesc, uint64_t bdesc, int accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n\t}"
+      : PTD_F8(0), PTD_F8(8), PTD_F8(16), PTD_F8(24)
+      : "l"(adesc), "l"(bdesc), "r"(accumulate));
+}
+// D[64 x 128] (+)= A[64 x 16] * B[128 x 16]^T, fp32 accumulators in d[64]
+__device__ __forceinline__ void wgmma_n128(float* d, uint64_t adesc, uint64_t bdesc, int accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n\t}"
+      : PTD_F8(0), PTD_F8(8), PTD_F8(16), PTD_F8(24), PTD_F8(32), PTD_F8(40), PTD_F8(48), PTD_F8(56)
+      : "l"(adesc), "l"(bdesc), "r"(accumulate));
+}
+#undef PTD_F8
+
+// keeps the compiler from moving accumulator reads / writes across the asynchronous wgmma window
+template <int N> __device__ __forceinline__ void fence_regs(float (&d)[N]) {
 #pragma unroll
-  for (int s = 16; s >= 1; s >>= 1) {
-    const bool upper = (lane & s) != 0;
-#pragma unroll
-    for (int j = 0; j < s; ++j) {
-      const float send = upper ? v[j] : v[j + s];
-      const float keep = upper ? v[j + s] : v[j];
-      v[j] = keep + __shfl_xor_sync(0xffffffffu, send, s);
-    }
-  }
-  return v[0];
+  for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
 template <int BLOCK_N>
-__global__ void __launch_bounds__(kGemmThreads) gemm_bnstats_kernel(const __grid_constant__ CUtensorMap tmap_a,
-                                                                    const __grid_constant__ CUtensorMap tmap_b,
-                                                                    __nv_bfloat16* __restrict__ C, float* __restrict__ gsum, int M, int N, int K) {
-  constexpr int kABytes = kBlockM * kBlockK * 2;
-  constexpr int kBBytes = BLOCK_N * kBlockK * 2;
+__global__ void __launch_bounds__(kGemmThreads, 1) gemm_bnstats_kernel(const __grid_constant__ CUtensorMap tmap_a,
+                                                                       const __grid_constant__ CUtensorMap tmap_b,
+                                                                       const __grid_constant__ CUtensorMap tmap_c,
+                                                                       float* __restrict__ part, int N, int K, int m_tiles,
+                                                                       int n_tiles, int ctas_per_n) {
+  using Cfg = GemmCfg<BLOCK_N>;
+  constexpr int kStages = Cfg::kStages;
+  constexpr int kInstN = BLOCK_N >= 128 ? 128 : 64;                  // wgmma N per instruction
+  constexpr int kBoxes = BLOCK_N / 64;                               // 64-column output boxes
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  uint8_t* smem_a = smem;                                   // [kStages][128 x 64] bf16, 128B swizzle
-  uint8_t* smem_b = smem + kStages * kABytes;               // [kStages][BLOCK_N x 64]
-  float* smem_stats = reinterpret_cast<float*>(smem_b + kStages * kBBytes);   // [4 warps][2][BLOCK_N]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem_stats + 4 * 2 * BLOCK_N);
-  uint64_t* full_bar = bars;                                // [kStages]
-  uint64_t* empty_bar = bars + kStages;                     // [kStages]
-  uint64_t* tmem_full_bar = bars + 2 * kStages;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * kStages + 1);
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int m0 = blockIdx.x * kBlockM, n0 = blockIdx.y * BLOCK_N;
-  const int num_kb = K / kBlockK;
-
-  if (warp == 0 && lane == 0) {
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmap_a) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmap_b) : "memory");
-    for (int s = 0; s < kStages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
-    mbar_init(tmem_full_bar, 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 1) {                                           // TMEM: BLOCK_N fp32 columns x 128 lanes
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "n"(BLOCK_N) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *tmem_slot;
-
-  if (warp == 0) {
-    // ===== TMA producer
-    if (elect_one()) {
-      for (int kb = 0; kb < num_kb; ++kb) {
-        const int s = kb % kStages;
-        if (kb >= kStages) mbar_wait(&empty_bar[s], ((kb / kStages) - 1) & 1);
-        mbar_expect_tx(&full_bar[s], kABytes + kBBytes);
-        tma_load_2d(smem_a + s * kABytes, &tmap_a, &full_bar[s], kb * kBlockK, m0);
-        tma_load_2d(smem_b + s * kBBytes, &tmap_b, &full_bar[s], kb * kBlockK, n0);
-      }
-    }
-  } else if (warp == 1) {
-    // ===== MMA issuer
-    // instruction descriptor: D=f32, A=B=bf16, both K-major, N>>3, M>>4
-    constexpr uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(BLOCK_N >> 3) << 17) | ((uint32_t)(kBlockM >> 4) << 24);
-    for (int kb = 0; kb < num_kb; ++kb) {
-      const int s = kb % kStages;
-      mbar_wait(&full_bar[s], (kb / kStages) & 1);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      if (elect_one()) {
-        const uint64_t adesc = umma_desc(smem_a + s * kABytes), bdesc = umma_desc(smem_b + s * kBBytes);
-#pragma unroll
-        for (int k = 0; k < kBlockK / 16; ++k)   // UMMA_K = 16 bf16 = 32 bytes = +2 in the (>>4) start-address field
-          umma_f16(tmem_base, adesc + 2 * k, bdesc + 2 * k, idesc, (kb | k) != 0);
-        umma_commit(&empty_bar[s]);              // frees the smem stage once these MMAs have read it
-        if (kb == num_kb - 1) umma_commit(tmem_full_bar);
-      }
-      __syncwarp();
-    }
-  } else {
-    // ===== epilogue: warp w may only touch TMEM lanes [32*(w%4), 32*(w%4)+32)
-    const int q = warp & 3;
-    const int row = m0 + q * 32 + lane;
-    mbar_wait(tmem_full_bar, 0);
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    float* my_stats = smem_stats + (warp - 2) * 2 * BLOCK_N;
-#pragma unroll 1
-    for (int c = 0; c < BLOCK_N / 32; ++c) {
-      uint32_t r[32];
-      tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(c * 32), r);
-      float v[32], w[32];
-#pragma unroll
-      for (int j = 0; j < 32; ++j) { v[j] = __uint_as_float(r[j]); w[j] = v[j] * v[j]; }
-      if (row < M) {
-        __nv_bfloat16* dst = C + (int64_t)row * N + n0 + c * 32;
-#pragma unroll
-        for (int j = 0; j < 32; j += 8) {
-          V4 o{Wire<__nv_bfloat16>::pack2(v[j], v[j + 1]), Wire<__nv_bfloat16>::pack2(v[j + 2], v[j + 3]),
-               Wire<__nv_bfloat16>::pack2(v[j + 4], v[j + 5]), Wire<__nv_bfloat16>::pack2(v[j + 6], v[j + 7])};
-          st_v4(dst + j, o);
-        }
-      }
-      // rows >= M were zero-filled by TMA: they contribute 0 to both sums
-      const float cs = column_reduce(v, lane), cq = column_reduce(w, lane);
-      my_stats[c * 32 + lane] = cs;
-      my_stats[BLOCK_N + c * 32 + lane] = cq;
-    }
-    asm volatile("bar.sync 1, 128;" ::: "memory");           // the four epilogue warps only
-    for (int i = threadIdx.x - 64; i < 2 * BLOCK_N; i += 128) {
-      const float s4 = smem_stats[i] + smem_stats[2 * BLOCK_N + i] + smem_stats[4 * BLOCK_N + i] + smem_stats[6 * BLOCK_N + i];
-      const int half = i >= BLOCK_N, col = i - half * BLOCK_N;
-      atomicAdd(&gsum[half * N + n0 + col], s4);
-    }
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 1) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(BLOCK_N) : "memory");
-  }
-}
-
-// ====================================================================================================================
-// Version 2: persistent CTAs, 4-stage TMA ring, DOUBLE-BUFFERED TMEM accumulators and 8 epilogue warps.
-//   * one CTA per SM loops over output tiles with a FIXED n-tile (so the per-channel partial sums live in shared
-//     memory for the CTA's lifetime and reach global memory once), m-tiles strided by the number of CTAs per n-tile;
-//     CTAs with adjacent ids share the same m-tile sequence => the A tile is fetched from HBM once and hit in L2 by
-//     the other n-tiles;
-//   * the MMA warp fills TMEM buffer (j & 1) for tile j while the epilogue warps drain buffer ((j-1) & 1):
-//     tmem_full[2] / tmem_empty[2] mbarriers, the TMA producer runs up to 4 k-blocks ahead across tile boundaries;
-//   * epilogue: two warps per TMEM lane quadrant split the 32-column chunks; the next chunk's tcgen05.ld is issued
-//     before the current chunk is reduced / packed / stored.
-constexpr int kStagesV2 = 3;
-constexpr int kEpiWarps = 8;
-constexpr int kThreadsV2 = 64 + kEpiWarps * 32;
-
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void tmem_ld32_nowait(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-        "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]),
-        "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-        "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-}
-
-template <int BLOCK_N>
-__global__ void __launch_bounds__(kThreadsV2, 1) gemm_bnstats_persistent_kernel(const __grid_constant__ CUtensorMap tmap_a,
-                                                                                const __grid_constant__ CUtensorMap tmap_b,
-                                                                                const __grid_constant__ CUtensorMap tmap_c,
-                                                                                float* __restrict__ gsum, int M, int N, int K, int m_tiles,
-                                                                                int n_tiles, int ctas_per_n) {
-  constexpr int kABytes = kBlockM * kBlockK * 2;
-  constexpr int kBBytes = BLOCK_N * kBlockK * 2;
-  constexpr int kChunks = BLOCK_N / 32;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  uint8_t* smem_a = smem;
-  uint8_t* smem_b = smem + kStagesV2 * kABytes;
-  uint8_t* smem_stage = smem_b + kStagesV2 * kBBytes;                           // per epilogue warp: 2 x 4 KB bf16 staging
-  float* smem_stats = reinterpret_cast<float*>(smem_stage + kEpiWarps * 8192);   // [4 quadrants][2][BLOCK_N]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem_stats + 4 * 2 * BLOCK_N);
-  uint64_t* full_bar = bars;
-  uint64_t* empty_bar = bars + kStagesV2;
-  uint64_t* tmem_full = bars + 2 * kStagesV2;      // [2]
-  uint64_t* tmem_empty = bars + 2 * kStagesV2 + 2; // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * kStagesV2 + 4);
+  uint8_t* smem_a = smem;                                            // [kStages][128 x 64] bf16, 128B swizzle
+  uint8_t* smem_b = smem_a + kStages * Cfg::kABytes;                 // [kStages][BLOCK_N x 64]
+  uint8_t* smem_c = smem_b + kStages * Cfg::kBBytes;                 // [2 warpgroups][kBoxes][64 x 64] bf16, 128B swizzle
+  float* smem_stats = reinterpret_cast<float*>(smem_c + Cfg::kCBytes);   // [2 warpgroups][s0 s1 q0 q1][128 threads]
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem_stats + Cfg::kStatFloats);
+  uint64_t* empty_bar = full_bar + kStages;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int n_tile = blockIdx.x % n_tiles;           // fixed for this CTA
@@ -266,139 +135,113 @@ __global__ void __launch_bounds__(kThreadsV2, 1) gemm_bnstats_persistent_kernel(
   const int n0 = n_tile * BLOCK_N;
   const int num_kb = K / kBlockK;
 
-  if (warp == 0 && lane == 0) {
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmap_a) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmap_b) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmap_c) : "memory");
-    for (int s = 0; s < kStagesV2; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
-    for (int b = 0; b < 2; ++b) { mbar_init(&tmem_full[b], 1); mbar_init(&tmem_empty[b], kEpiWarps); }
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < kStages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], kConsumerThreads / 32); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "n"(2 * BLOCK_N) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  for (int i = threadIdx.x; i < 4 * 2 * BLOCK_N; i += blockDim.x) smem_stats[i] = 0.f;
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
-    // ===== TMA producer (runs ahead across tile boundaries)
-    if (elect_one()) {
+  if (warp == kConsumerThreads / 32) {
+    // ===== TMA producer
+    if (lane == 0) {
+      asm volatile("prefetch.tensormap [%0];" ::"l"(&tmap_a) : "memory");
+      asm volatile("prefetch.tensormap [%0];" ::"l"(&tmap_b) : "memory");
       uint32_t it = 0;
       for (int mt = m_first; mt < m_tiles; mt += ctas_per_n) {
         for (int kb = 0; kb < num_kb; ++kb, ++it) {
-          const int s = it % kStagesV2;
-          mbar_wait(&empty_bar[s], ((it / kStagesV2) & 1) ^ 1);
-          mbar_expect_tx(&full_bar[s], kABytes + kBBytes);
-          tma_load_2d(smem_a + s * kABytes, &tmap_a, &full_bar[s], kb * kBlockK, mt * kBlockM);
-          tma_load_2d(smem_b + s * kBBytes, &tmap_b, &full_bar[s], kb * kBlockK, n0);
+          const int s = it % kStages;
+          mbar_wait(&empty_bar[s], ((it / kStages) & 1) ^ 1);
+          mbar_expect_tx(&full_bar[s], Cfg::kABytes + Cfg::kBBytes);
+          tma_load_2d(smem_a + s * Cfg::kABytes, &tmap_a, &full_bar[s], kb * kBlockK, mt * kBlockM);
+          tma_load_2d(smem_b + s * Cfg::kBBytes, &tmap_b, &full_bar[s], kb * kBlockK, n0);
         }
       }
     }
-  } else if (warp == 1) {
-    // ===== MMA issuer
-    constexpr uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(BLOCK_N >> 3) << 17) | ((uint32_t)(kBlockM >> 4) << 24);
-    uint32_t it = 0, j = 0;
-    for (int mt = m_first; mt < m_tiles; mt += ctas_per_n, ++j) {
-      const uint32_t buf = j & 1;
-      mbar_wait(&tmem_empty[buf], ((j >> 1) & 1) ^ 1);        // the epilogue has drained this accumulator buffer
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      for (int kb = 0; kb < num_kb; ++kb, ++it) {
-        const int s = it % kStagesV2;
-        mbar_wait(&full_bar[s], (it / kStagesV2) & 1);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        if (elect_one()) {
-          const uint64_t adesc = umma_desc(smem_a + s * kABytes), bdesc = umma_desc(smem_b + s * kBBytes);
+    return;
+  }
+
+  // ===== consumers: warpgroup wg computes rows [64 wg, 64 wg + 64) of every tile
+  const int wg = warp >> 2, t = threadIdx.x & 127, w = warp & 3;
+  uint8_t* stg = smem_c + wg * (Cfg::kCBytes / 2);
+  float acc[BLOCK_N / 2] = {};
+  // accumulator acc[4j + e] holds row 16w + (lane >> 2) + 8 (e >> 1), column 8j + 2 (lane & 3) + (e & 1) of the
+  // warpgroup's 64 x BLOCK_N block, whichever wgmma width produced it
+  const int r0 = 16 * w + (lane >> 2);
+  // statistics: thread t owns column pair p = t % (BLOCK_N / 2) over a 1 / kParts share of the 64 rows
+  constexpr int kPairs = BLOCK_N / 2, kParts = 128 / kPairs, kRows = 64 / kParts;
+  const int p = t % kPairs, rpart = t / kPairs;
+  const int p_box = p >> 5, p_gran = (p & 31) >> 2, p_byte = (p & 3) * 4;
+  float s0 = 0.f, s1 = 0.f, q0 = 0.f, q1 = 0.f;
+
+  uint32_t it = 0;
+  for (int mt = m_first; mt < m_tiles; mt += ctas_per_n) {
+    for (int kb = 0; kb < num_kb; ++kb, ++it) {
+      const int s = it % kStages;
+      mbar_wait(&full_bar[s], (it / kStages) & 1);
+      const uint64_t adesc = gmma_desc(smem_a + s * Cfg::kABytes + wg * 64 * 128);
+      const uint64_t bdesc = gmma_desc(smem_b + s * Cfg::kBBytes);
+      fence_regs(acc);
+      asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
 #pragma unroll
-          for (int k = 0; k < kBlockK / 16; ++k)
-            umma_f16(tmem_base + buf * BLOCK_N, adesc + 2 * k, bdesc + 2 * k, idesc, (kb | k) != 0);
-          umma_commit(&empty_bar[s]);
-          if (kb == num_kb - 1) umma_commit(&tmem_full[buf]);
+      for (int k = 0; k < kBlockK / 16; ++k) {
+#pragma unroll
+        for (int h = 0; h < BLOCK_N / kInstN; ++h) {
+          // B rows [h * kInstN, ...) start h * kInstN * 128 bytes further: +8 * kInstN in the (>>4) address field
+          if constexpr (kInstN == 128) wgmma_n128(acc + h * 64, adesc + 2 * k, bdesc + h * 8 * kInstN + 2 * k, (kb | k) != 0);
+          else wgmma_n64(acc + h * 32, adesc + 2 * k, bdesc + h * 8 * kInstN + 2 * k, (kb | k) != 0);
         }
-        __syncwarp();
       }
+      asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
+      asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
+      fence_regs(acc);
+      if (lane == 0) mbar_arrive(&empty_bar[s]);                   // this warp has finished reading the stage
     }
-  } else {
-    // ===== epilogue: warps 2..9; quadrant q = warp & 3 (hardware: a warp may only read TMEM lanes 32*(warp%4)..+31),
-    // half h picks the even / odd 32-column chunks
-    const int q = warp & 3, h = (warp - 2) >> 2;
-    float* my_stats = smem_stats + q * 2 * BLOCK_N;
-    // Per step a warp drains 32 rows x 64 columns: TMEM -> registers -> bf16 -> shared memory in the TMA SWIZZLE_128B
-    // layout (row owner = lane; 16-byte granule k of row i lands in slot k ^ (i & 7): conflict-free for the row-owner
-    // writes AND for the column-owner reads below) -> ONE cp.async.bulk.tensor store per step (coalesced, off the LSU,
-    // clipped at the M tail by the tensor map).  The statistics are taken from the bf16-rounded values - exactly what
-    // a separate BatchNorm pass over the stored tensor would see - by column owners (lane = 2 adjacent columns).
-    uint8_t* st_base = smem_stage + (warp - 2) * 8192;         // 2 x 4 KB
-    constexpr int kSteps = BLOCK_N / 64;
-    uint32_t nstore = 0;
-    uint32_t j = 0;
-    for (int mt = m_first; mt < m_tiles; mt += ctas_per_n, ++j) {
-      const uint32_t buf = j & 1;
-      mbar_wait(&tmem_full[buf], (j >> 1) & 1);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      const uint32_t tbase = tmem_base + buf * BLOCK_N + ((uint32_t)(q * 32) << 16);
-#pragma unroll 1
-      for (int st = h; st < kSteps; st += 2) {
-        uint32_t r0[32], r1[32];
-        tmem_ld32_nowait(tbase + st * 64, r0);
-        tmem_ld32_nowait(tbase + st * 64 + 32, r1);
-        // the staging buffer we are about to fill was handed to TMA two stores ago: wait until it has been read
-        uint8_t* stg = st_base + (nstore & 1) * 4096;
-        if (lane == 0) asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory");
-        __syncwarp();
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+
+    // ---- epilogue: the staging tile may be refilled once the previous tile's TMA store has read it
+    if (t == 0) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
+    named_barrier(1 + wg, 128);
 #pragma unroll
-        for (int k = 0; k < 8; ++k) {                          // 8 granules of 8 bf16 per 128-byte row
-          const uint32_t* src = k < 4 ? r0 : r1;
-          const int o = (k & 3) * 8;
-          V4 g{Wire<__nv_bfloat16>::pack2(__uint_as_float(src[o]), __uint_as_float(src[o + 1])),
-               Wire<__nv_bfloat16>::pack2(__uint_as_float(src[o + 2]), __uint_as_float(src[o + 3])),
-               Wire<__nv_bfloat16>::pack2(__uint_as_float(src[o + 4]), __uint_as_float(src[o + 5])),
-               Wire<__nv_bfloat16>::pack2(__uint_as_float(src[o + 6]), __uint_as_float(src[o + 7]))};
-          *reinterpret_cast<V4*>(stg + lane * 128 + ((k ^ (lane & 7)) << 4)) = g;
-        }
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes -> visible to the TMA engine
-        __syncwarp();
-        if (lane == 0) {
-          asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
-                       ::"l"(&tmap_c), "r"(smem_u32(stg)), "r"(n0 + st * 64), "r"(mt * kBlockM + q * 32) : "memory");
-          asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-        }
-        ++nstore;
-        // column owners: lane L sums columns 2L and 2L+1 over the 32 rows (one bf16x2 word per row)
-        float s0 = 0.f, s1 = 0.f, q0 = 0.f, q1 = 0.f;
-        const int gsel = lane >> 2, within = (lane & 3) << 2;
-#pragma unroll
-        for (int rr = 0; rr < 32; ++rr) {
-          const uint32_t wv = *reinterpret_cast<const uint32_t*>(stg + rr * 128 + ((gsel ^ (rr & 7)) << 4) + within);
-          const float2 f = Wire<__nv_bfloat16>::unpack2(wv);
-          s0 += f.x; q0 += f.x * f.x;
-          s1 += f.y; q1 += f.y * f.y;
-        }
-        float* ms = my_stats + st * 64 + 2 * lane;             // (quadrant, column) is owned by exactly one lane of one warp
-        ms[0] += s0; ms[1] += s1;
-        ms[BLOCK_N] += q0; ms[BLOCK_N + 1] += q1;
-      }
-      // this warp no longer needs the TMEM buffer (every epilogue warp arrives once per tile, also the idle ones)
-      asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-      if (lane == 0) mbar_arrive(&tmem_empty[buf]);
+    for (int j = 0; j < BLOCK_N / 8; ++j) {
+      // 16-byte granule g of row r sits at slot g ^ (r & 7) (the TMA SWIZZLE_128B layout): conflict-free here and below
+      uint8_t* box = stg + (j >> 3) * 8192 + (lane & 3) * 4;
+      const int g = j & 7;
+      *reinterpret_cast<uint32_t*>(box + r0 * 128 + ((g ^ (r0 & 7)) << 4)) = Wire<__nv_bfloat16>::pack2(acc[4 * j], acc[4 * j + 1]);
+      *reinterpret_cast<uint32_t*>(box + (r0 + 8) * 128 + ((g ^ (r0 & 7)) << 4)) =
+          Wire<__nv_bfloat16>::pack2(acc[4 * j + 2], acc[4 * j + 3]);
     }
-    if (lane == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");   // outstanding output stores have landed
-    __syncwarp();
-    asm volatile("bar.sync 1, 256;" ::: "memory");             // the eight epilogue warps
-    for (int i = threadIdx.x - 64; i < 2 * BLOCK_N; i += kEpiWarps * 32) {
-      const float s4 = smem_stats[i] + smem_stats[2 * BLOCK_N + i] + smem_stats[4 * BLOCK_N + i] + smem_stats[6 * BLOCK_N + i];
-      const int half = i >= BLOCK_N, col = i - half * BLOCK_N;
-      atomicAdd(&gsum[half * N + n0 + col], s4);
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");     // generic-proxy writes -> visible to the TMA engine
+    named_barrier(1 + wg, 128);
+    if (t == 0) {
+#pragma unroll
+      for (int b = 0; b < kBoxes; ++b)
+        asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
+                     ::"l"(&tmap_c), "r"(smem_u32(stg + b * 8192)), "r"(n0 + b * 64), "r"(mt * kBlockM + wg * 64) : "memory");
+      asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+    }
+    // The statistics are taken from the bf16-rounded values - exactly what a separate BatchNorm pass over the stored
+    // tensor would see.  Rows past M were zero-filled by TMA: they contribute 0 to both sums.
+    const uint8_t* src = stg + p_box * 8192 + p_byte;
+#pragma unroll 8
+    for (int r = rpart * kRows; r < rpart * kRows + kRows; ++r) {
+      const float2 f = Wire<__nv_bfloat16>::unpack2(*reinterpret_cast<const uint32_t*>(src + r * 128 + ((p_gran ^ (r & 7)) << 4)));
+      s0 += f.x; q0 += f.x * f.x;
+      s1 += f.y; q1 += f.y * f.y;
     }
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 1) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(2 * BLOCK_N) : "memory");
+  if (t == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");   // outstanding output stores have landed
+  // Fixed-order combine (no atomics, so the statistics are the same bits on every run): the per-thread sums go to shared
+  // memory, then one thread per (sum, column) adds the warpgroups and row parts in order and writes this CTA's row of
+  // the partials, part[m_first][0:N] (sums) / [N:2N] (sums of squares); combine_partials() adds the rows.
+  float* my = smem_stats + wg * 4 * 128 + t;
+  my[0] = s0; my[128] = s1; my[256] = q0; my[384] = q1;
+  named_barrier(3, kConsumerThreads);
+  for (int i = threadIdx.x; i < 2 * BLOCK_N; i += kConsumerThreads) {
+    const int half = i >= BLOCK_N, col = i - half * BLOCK_N;
+    const int pair = col >> 1, which = half * 2 + (col & 1);        // which: s0, s1, q0, q1
+    float v = 0.f;
+    for (int w2 = 0; w2 < 2; ++w2)
+      for (int pt = 0; pt < kParts; ++pt) v += smem_stats[w2 * 4 * 128 + which * 128 + pt * kPairs + pair];
+    part[(size_t)m_first * 2 * N + half * N + n0 + col] = v;
   }
 }
 
@@ -417,68 +260,40 @@ static EncodeTiledFn encode_fn() {
   return fn;
 }
 
-// output matrix: 32-row x 64-column boxes in the 128-byte swizzle layout the epilogue writes
-static CUtensorMap make_map(const void* ptr, int64_t rows, int64_t cols, int box_rows);
-static EncodeTiledFn encode_fn();
-static CUtensorMap make_store_map(const void* ptr, int64_t rows, int64_t cols) {
-  CUtensorMap m;
-  cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
-  cuuint64_t strides[1] = {(cuuint64_t)cols * 2};
-  cuuint32_t box[2] = {64, 32};
-  cuuint32_t estr[2] = {1, 1};
-  CUresult r = encode_fn()(&m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(ptr), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                           CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  TORCH_CHECK(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled(store) failed: ", (int)r);
-  return m;
-}
-
 // row-major [rows, cols] bf16 matrix, box = box_rows x 64 columns, 128-byte swizzle
-static CUtensorMap make_map(const void* ptr, int64_t rows, int64_t cols, int box_rows) {
+static CUtensorMap make_map(const void* ptr, int64_t rows, int64_t cols, int box_rows, CUtensorMapL2promotion promo) {
   CUtensorMap m;
   cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
   cuuint64_t strides[1] = {(cuuint64_t)cols * 2};
   cuuint32_t box[2] = {(cuuint32_t)kBlockK, (cuuint32_t)box_rows};
   cuuint32_t estr[2] = {1, 1};
   CUresult r = encode_fn()(&m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(ptr), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                           CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+                           CU_TENSOR_MAP_SWIZZLE_128B, promo, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   TORCH_CHECK(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled failed: ", (int)r);
   return m;
 }
 
 template <int BLOCK_N>
 static void launch_gemm(const at::Tensor& a, const at::Tensor& b, at::Tensor& c, at::Tensor& gsum, int M, int N, int K) {
-  constexpr size_t smem = 1024 + kStages * (kBlockM * kBlockK * 2 + BLOCK_N * kBlockK * 2) + 4 * 2 * BLOCK_N * sizeof(float) + 64;
+  constexpr int smem = GemmCfg<BLOCK_N>::kSmem;
   static bool configured[64] = {};                 // the attribute is per device (DataParallel drives several from one process)
   const int dev = a.get_device();
   if (!configured[dev & 63]) {
-    C10_CUDA_CHECK(cudaFuncSetAttribute(gemm_bnstats_kernel<BLOCK_N>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    C10_CUDA_CHECK(cudaFuncSetAttribute(gemm_bnstats_kernel<BLOCK_N>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     configured[dev & 63] = true;
   }
-  const CUtensorMap ma = make_map(a.data_ptr(), M, K, kBlockM), mb = make_map(b.data_ptr(), N, K, BLOCK_N);
-  dim3 grid((M + kBlockM - 1) / kBlockM, N / BLOCK_N);
-  gemm_bnstats_kernel<BLOCK_N><<<grid, kGemmThreads, smem, at::cuda::getCurrentCUDAStream()>>>(
-      ma, mb, reinterpret_cast<__nv_bfloat16*>(c.data_ptr()), gsum.data_ptr<float>(), M, N, K);
-  C10_CUDA_KERNEL_LAUNCH_CHECK();
-}
-
-template <int BLOCK_N>
-static void launch_gemm_v2(const at::Tensor& a, const at::Tensor& b, at::Tensor& c, at::Tensor& gsum, int M, int N, int K) {
-  constexpr size_t smem = 1024 + kStagesV2 * (kBlockM * kBlockK * 2 + BLOCK_N * kBlockK * 2) + kEpiWarps * 8192 + 4 * 2 * BLOCK_N * sizeof(float) + 128;
-  static bool configured[64] = {};                 // the attribute is per device (DataParallel drives several from one process)
-  const int dev = a.get_device();
-  if (!configured[dev & 63]) {
-    C10_CUDA_CHECK(cudaFuncSetAttribute(gemm_bnstats_persistent_kernel<BLOCK_N>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    configured[dev & 63] = true;
-  }
-  const CUtensorMap ma = make_map(a.data_ptr(), M, K, kBlockM), mb = make_map(b.data_ptr(), N, K, BLOCK_N);
-  const CUtensorMap mc = make_store_map(c.data_ptr(), M, N);
+  const CUtensorMap ma = make_map(a.data_ptr(), M, K, kBlockM, CU_TENSOR_MAP_L2_PROMOTION_L2_256B);
+  const CUtensorMap mb = make_map(b.data_ptr(), N, K, BLOCK_N, CU_TENSOR_MAP_L2_PROMOTION_L2_256B);
+  const CUtensorMap mc = make_map(c.data_ptr(), M, N, 64, CU_TENSOR_MAP_L2_PROMOTION_NONE);   // 64 x 64 store boxes
   const int m_tiles = (M + kBlockM - 1) / kBlockM, n_tiles = N / BLOCK_N;
   const int sms = at::cuda::getCurrentDeviceProperties()->multiProcessorCount;
   const int ctas_per_n = std::max(1, std::min(m_tiles, sms / n_tiles));
   const int grid = ctas_per_n * n_tiles;
-  gemm_bnstats_persistent_kernel<BLOCK_N><<<grid, kThreadsV2, smem, at::cuda::getCurrentCUDAStream()>>>(
-      ma, mb, mc, gsum.data_ptr<float>(), M, N, K, m_tiles, n_tiles, ctas_per_n);
+  cudaStream_t st = at::cuda::getCurrentCUDAStream();
+  at::Tensor part = at::empty({ctas_per_n, 2 * N}, gsum.options());
+  gemm_bnstats_kernel<BLOCK_N><<<grid, kGemmThreads, smem, st>>>(ma, mb, mc, part.data_ptr<float>(), N, K, m_tiles, n_tiles, ctas_per_n);
   C10_CUDA_KERNEL_LAUNCH_CHECK();
+  combine_partials(part.data_ptr<float>(), ctas_per_n, 2 * N, gsum.data_ptr<float>(), st);
 }
 
 // x: [B, K, H, W] channels_last bf16; weight: [N, K, 1, 1] bf16 (any dense layout); gsum: zeroed float[2N].
@@ -497,13 +312,6 @@ at::Tensor conv1x1_bnstats(const at::Tensor& x, const at::Tensor& weight, at::Te
   at::Tensor y = at::empty({x.size(0), N, x.size(2), x.size(3)}, x.options().memory_format(at::MemoryFormat::ChannelsLast));
   const int M = (int)M64;
   static const int max_bn = getenv("PTD_GEMM_BLOCK_N") ? atoi(getenv("PTD_GEMM_BLOCK_N")) : 256;
-  static const int version = getenv("PTD_GEMM_V") ? atoi(getenv("PTD_GEMM_V")) : 2;
-  if (version >= 2) {
-    if (N % 256 == 0 && max_bn >= 256) launch_gemm_v2<256>(x, w2, y, gsum, M, N, K);
-    else if (N % 128 == 0 && max_bn >= 128) launch_gemm_v2<128>(x, w2, y, gsum, M, N, K);
-    else launch_gemm_v2<64>(x, w2, y, gsum, M, N, K);
-    return y;
-  }
   if (N % 256 == 0 && max_bn >= 256) launch_gemm<256>(x, w2, y, gsum, M, N, K);
   else if (N % 128 == 0 && max_bn >= 128) launch_gemm<128>(x, w2, y, gsum, M, N, K);
   else launch_gemm<64>(x, w2, y, gsum, M, N, K);

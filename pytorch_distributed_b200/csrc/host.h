@@ -1,5 +1,6 @@
 // Host-side declarations shared by the .cu / .cpp translation units and the bindings.
 #pragma once
+#include <cuda_runtime_api.h>
 #include <torch/extension.h>
 
 #include <cstdint>
@@ -42,6 +43,8 @@ void amp_update_scale(at::Tensor scale, at::Tensor growth_tracker, at::Tensor fo
                       int64_t interval, at::Tensor hyper);
 
 // ---- bn_act.cu
+// gsum[0:n] += the rows part[0:nblocks][0:n] summed in a fixed order (deterministic cross-CTA reduction)
+void combine_partials(const float* part, int nblocks, int n, float* gsum, cudaStream_t st);
 std::vector<at::Tensor> bn_act_forward(const at::Tensor& x, const c10::optional<at::Tensor>& residual, const at::Tensor& weight,
                                        const at::Tensor& bias, at::Tensor running_mean, at::Tensor running_var,
                                        c10::optional<at::Tensor> num_batches_tracked, bool training, double momentum, double eps, bool relu,
@@ -61,7 +64,7 @@ std::vector<at::Tensor> stem_forward_pre(const at::Tensor& x, const at::Tensor& 
 std::vector<at::Tensor> stem_backward(const at::Tensor& dp, const at::Tensor& x, const at::Tensor& code, const at::Tensor& weight,
                                       const at::Tensor& saved, at::Tensor work);
 
-// ---- gemm_bnstats.cu (tcgen05 / TMA / TMEM)
+// ---- gemm_bnstats.cu (wgmma / TMA)
 at::Tensor conv1x1_bnstats(const at::Tensor& x, const at::Tensor& weight, at::Tensor gsum);
 
 // ---- stem_conv.cu

@@ -2,7 +2,7 @@
 // antialiased bilinear resample, horizontal flip -> planar uint8 batches written straight into (pinned) ring slots.
 //
 // Role: the reference feeds its loops with torch DataLoader worker PROCESSES running PIL per sample
-// (/root/reference/distributed.py:160-195, transforms at :165-172 and :183-188).  At ~11k images/s per B200 that host
+// (reference distributed.py:160-195, transforms at :165-172 and :183-188).  At thousands of images/s per GPU that host
 // path cannot keep a node busy, so the steady-state loader here is native: no Python, no pickling, no per-sample
 // allocation in the hot loop.  JPEG decoding happens once, offline (tools/make_shards.py).  The device side is the
 // existing fused normalise/cast/NHWC kernel (csrc/data_ops.cu), fed with the uint8 NCHW batches produced here.

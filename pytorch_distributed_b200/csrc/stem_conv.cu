@@ -1,10 +1,9 @@
-// ResNet stem convolution (7x7, stride 2, pad 3, C_in = 3) as im2col + the tcgen05 GEMM of gemm_bnstats.cu (sm_100a).
+// ResNet stem convolution (7x7, stride 2, pad 3, C_in = 3) as im2col + the wgmma GEMM of gemm_bnstats.cu (sm_90a).
 //
-// cuDNN serves this layer with legacy sm80 kernels (C_in = 3 fits no tensor-core tile): 1.5 ms forward + 0.8 ms wgrad per
-// 256-image step, 10 % of the whole ResNet-50 step (profiles/step_breakdown_r1.md; padding C_in to 4 or 8 does not help,
+// cuDNN serves this layer with legacy kernels (C_in = 3 fits no tensor-core tile; padding C_in to 4 or 8 does not help,
 // tools/conv_stem_probe.py).  The layer is only 60 GFLOP; written as a GEMM it is bound by its 411 MB output:
 //   A[M, 192]  = im2col(x)        M = N*OH*OW output pixels, one 384-byte row per pixel        (this file)
-//   Y[M, 64]   = A x Wp^T         persistent tcgen05 GEMM, BatchNorm statistics in its epilogue  (gemm_bnstats.cu)
+//   Y[M, 64]   = A x Wp^T         persistent wgmma GEMM, BatchNorm statistics in its epilogue    (gemm_bnstats.cu)
 //   dWp[64,192]= dY^T x A         library GEMM over the saved A                                  (ops/stem_conv.py)
 // K ordering of a row: k = r*24 + s*3 + c for filter row r < 7, filter column s < 7, channel c < 3; positions with
 // s*3 + c >= 21 and k >= 168 are zero (the packed weights are zero there too).  A filter row is 21 CONTIGUOUS input
@@ -56,8 +55,7 @@ __global__ void __launch_bounds__(256) stem_im2col_scalar_kernel(const __nv_bflo
 }
 
 // One CTA per output row (n, oh).  The seven input rows the row's filter windows touch are staged in shared memory with
-// coalesced 16-byte loads (v1 gathered 2-byte elements from global memory: 196 instructions per granule, 75 % issue-active,
-// 2.2 TB/s - profiles/ncu_r2.md), each behind 16 zero elements and followed by 16 more, so the left / right image padding
+// coalesced 16-byte loads (gathering 2-byte elements from global memory costs ~200 instructions per granule), each behind 16 zero elements and followed by 16 more, so the left / right image padding
 // and the rows above / below the image are plain zeros in shared memory and EVERY granule takes the same path:
 // a filter row's 21 elements start at element (2*ow-3)*3 of the input row - an odd element index, i.e. 2 bytes past a
 // 4-byte word - so a granule is five aligned 32-bit shared loads and four PRMTs (hi half of word k | lo half of word k+1).

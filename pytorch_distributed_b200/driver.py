@@ -8,7 +8,7 @@ Hot-loop differences from the reference (/root/reference/distributed.py:242-276)
   * accuracy + ``barrier`` + 3x ``reduce_mean`` + 3x ``.item()`` collapse into ONE low-latency kernel whose result
     is fetched asynchronously (the meters lag the GPU by at most ``--print-freq`` iterations and are drained before
     every print), so the host never stalls the device inside the loop;
-  * gradient all-reduce, optimizer and loss scaling run through the fused sm_100a kernels.
+  * gradient all-reduce, optimizer and loss scaling run through the fused sm_90a kernels.
 Output contract (progress lines, `` * Acc@1`` summary, checkpoint files) is the reference's.
 """
 from __future__ import annotations
@@ -411,7 +411,7 @@ class HorovodStrategy(Strategy):
     """/root/reference/horovod_distributed.py: broadcast_parameters + DistributedOptimizer(compression=fp16)."""
     name = "horovod_distributed"
     overlap_optimizer = False   # horovod semantics: step() synchronises the handles first, then updates
-    cast_params = True          # bf16 model (tcgen05 conv / stem GEMM paths need bf16 weights); fp32 masters live in FusedSGD
+    cast_params = True          # bf16 model (wgmma conv / stem GEMM paths need bf16 weights); fp32 masters live in FusedSGD
     # the fusion dispatcher is a host thread: not capturable - unless the static schedule replaces it after the first step
     graph_capable = os.environ.get("PTD_HVD_STATIC", "1") == "1" and os.environ.get("HOROVOD_AUTOTUNE", "0") != "1"
 

@@ -4,7 +4,7 @@ Written from scratch; parameter / buffer names match torchvision's ResNet so the
 reference checkpoint layout (``state_dict`` of the unwrapped module,
 /root/reference/distributed.py:219-225) is interchangeable with torchvision.
 
-What is B200-specific: every BatchNorm is a :class:`BNAct` that runs the
+What is H100-specific: every BatchNorm is a :class:`BNAct` that runs the
 hand-written NHWC kernels in ``csrc/bn_act.cu`` (statistics pass + one fused
 normalise(+residual add)(+ReLU) pass, and the matching two-pass backward), so a
 bottleneck block issues 3 convs + 6 elementwise kernels instead of 3 convs + ~10.
@@ -19,19 +19,19 @@ from ..ops.conv_bn import conv1x1_bn_act
 from ..ops.stem import bn_relu_maxpool
 from ..ops.stem_conv import can_use_stem_gemm, stem_conv_bn_relu_maxpool
 
-# 1x1 conv -> BN pairs run as ONE tcgen05 GEMM with the BN statistics in its epilogue (ops/conv_bn.py,
-# profiles/gemm_bnstats_probe.md: -23 % vs cuDNN conv + separate statistics pass over the ResNet-50 shapes).
+# 1x1 conv -> BN pairs run as ONE wgmma GEMM with the BN statistics in its epilogue (ops/conv_bn.py; tools/gemm_probe.py
+# compares it with cuDNN conv + a separate statistics pass over the ResNet-50 shapes).
 # PTD_FUSED_CONV1X1=0 (or models.resnet.FUSED_CONV1X1 = False) restores cuDNN + bn_stats.
 import os as _os
 FUSED_CONV1X1 = _os.environ.get("PTD_FUSED_CONV1X1", "1") == "1"
 # A block's output has two consumers (the next block's first conv and its skip connection).  With SPLIT_RESGRAD the last
 # BNAct of a block hands out two aliases of its output, so the two gradients reach its backward separately and are
 # summed inside the BN-backward reduction pass (csrc/bn_act.cu: bn_act_backward2) instead of by an autograd add:
-# 7 instead of 9 tensor passes over the widest activations, -0.8 ms of 22 per step (profiles/bench_r2.md).
+# 7 instead of 9 tensor passes over the widest activations.
 # PTD_SPLIT_RESGRAD=0 restores the autograd add.
 SPLIT_RESGRAD = _os.environ.get("PTD_SPLIT_RESGRAD", "1") == "1"
-# Stem 7x7 convolution as im2col + the tcgen05 GEMM with fused BN statistics instead of cuDNN's legacy C_in = 3 kernels
-# (ops/stem_conv.py): cuDNN fprop 1.60 ms + wgrad 0.92 ms -> im2col 0.55 + GEMM 0.30 + wgrad GEMM 0.27 ms, -1.4 ms per step.
+# Stem 7x7 convolution as im2col + the wgmma GEMM with fused BN statistics instead of cuDNN's legacy C_in = 3 kernels
+# (ops/stem_conv.py; tools/stem_gemm_probe.py compares the two).
 # PTD_STEM_GEMM=0 restores cuDNN.
 STEM_GEMM = _os.environ.get("PTD_STEM_GEMM", "1") == "1"
 
@@ -71,7 +71,7 @@ class _Downsample(nn.Sequential):
     def __init__(self, cin, cout, stride, fused):
         super().__init__(_conv1x1(cin, cout, stride), BNAct(cout, relu=False, fused=fused))
 
-    def forward(self, x):        # stride-1 projections (layer1) take the tcgen05 GEMM + fused statistics path
+    def forward(self, x):        # stride-1 projections (layer1) take the wgmma GEMM + fused statistics path
         return conv1x1_bn_act(x, self[0], self[1], enabled=FUSED_CONV1X1)
 
 

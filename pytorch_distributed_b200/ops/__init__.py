@@ -1,1 +1,1 @@
-"""Hand-written sm_100a ops with PyTorch reference fall-backs (CPU / oracle)."""
+"""Hand-written sm_90a ops with PyTorch reference fall-backs (CPU / oracle)."""

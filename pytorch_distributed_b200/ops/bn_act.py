@@ -169,7 +169,7 @@ class _BnActFn(torch.autograd.Function):
             work, gen = ws.take(4 * nc)
         else:
             work, gen = torch.empty(0, dtype=torch.float32, device=x.device), -1
-        _ext.note_launch(1 if (stats_ready or not training) else 2)
+        _ext.note_launch(1 if (stats_ready or not training) else 3)   # stats + combine + apply
         y, saved, mask = C.bn_act_forward(x, residual, weight, bias, running_mean, running_var, nbt, training, momentum, eps, relu,
                                           need_grad, work[: 2 * nc] if training else work, stats_ready)
         ctx.relu = relu
@@ -198,7 +198,7 @@ class _BnActFn(torch.autograd.Function):
         work = ctx.work
         if work is None or (ctx.gen != -1 and ctx.gen != ctx.ws.generation):
             work = torch.zeros(2 * x.size(1), dtype=torch.float32, device=x.device)   # slice was recycled: use a fresh one
-        _ext.note_launch(2)
+        _ext.note_launch(3)                     # reduce + combine + apply
         if dy2 is not None:                     # add + mask + reductions in one pass; g doubles as the residual gradient
             dx, dres, dw, db = C.bn_act_backward2(dy, dy2, x, mask, weight, saved, ctx.relu, work)
         else:

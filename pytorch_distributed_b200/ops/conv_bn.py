@@ -1,7 +1,7 @@
 """``conv1x1_bn_act``: 1x1 convolution -> BatchNorm (+ residual) (+ ReLU) with the BN statistics produced by the GEMM.
 
-The convolution runs as a hand-written tcgen05 GEMM (``csrc/gemm_bnstats.cu``: TMA -> smem -> ``tcgen05.mma`` -> TMEM)
-whose epilogue reduces the per-channel sum / sum of squares from the fp32 accumulators, so BatchNorm only needs its
+The convolution runs as a hand-written wgmma GEMM (``csrc/gemm_bnstats.cu``: TMA -> smem -> ``wgmma.mma_async`` -> registers)
+whose epilogue reduces the per-channel sum / sum of squares of the stored bf16 output, so BatchNorm only needs its
 apply pass.  Backward: cuDNN dgrad / wgrad for the convolution, the fused BN backward kernels for the rest.
 Falls back to ``F.conv2d`` + :func:`bn_act` whenever the fast path does not apply (CPU, fp32/fp16, stride != 1, odd shapes).
 """
@@ -16,7 +16,7 @@ class _Conv1x1Stats(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x, weight, stats):
         from .. import _ext
-        _ext.note_launch()
+        _ext.note_launch(2)                     # GEMM + statistics combine
         y = _ext.lib().conv1x1_bnstats(x, weight, stats)
         ctx.save_for_backward(x, weight)
         return y

@@ -1,4 +1,4 @@
-"""FusedSGD: SGD with momentum / weight decay as hand-written sm_100a kernels (``csrc/optim.cu``).
+"""FusedSGD: SGD with momentum / weight decay as hand-written sm_90a kernels (``csrc/optim.cu``).
 
 Drop-in for ``torch.optim.SGD`` as used at /root/reference/distributed.py:153-156 and, together with
 :mod:`..parallel.amp`, for apex's patched optimizer + ``amp_C`` kernels (/root/reference/apex_distributed.py:211-216,330).

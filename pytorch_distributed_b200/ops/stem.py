@@ -27,7 +27,7 @@ class _StemFn(torch.autograd.Function):
             work, gen = ws.take(4 * nc)
         else:
             work, gen = torch.empty(0, dtype=torch.float32, device=x.device), -1
-        _ext.note_launch(2 if training else 1)
+        _ext.note_launch(3 if training else 1)
         y, saved, code = C.stem_forward(x, weight, bias, running_mean, running_var, nbt, training, momentum, eps, need_grad,
                                         work[: 2 * nc] if training else work)
         ctx.work = work[2 * nc:] if training else None
@@ -46,7 +46,7 @@ class _StemFn(torch.autograd.Function):
         work = ctx.work
         if work is None or (ctx.gen != -1 and ctx.gen != ctx.ws.generation):
             work = torch.zeros(2 * x.size(1), dtype=torch.float32, device=x.device)
-        _ext.note_launch(2)
+        _ext.note_launch(3)
         dx, dw, db = C.stem_backward(dy, x, code, weight, saved, work)
         return dx, dw, db, None, None, None, None, None, None, None
 

@@ -1,10 +1,10 @@
-"""ResNet stem convolution (7x7 / stride 2 / pad 3 / C_in = 3) as im2col + the tcgen05 GEMM, fused with the stem tail.
+"""ResNet stem convolution (7x7 / stride 2 / pad 3 / C_in = 3) as im2col + the wgmma GEMM, fused with the stem tail.
 
-cuDNN runs this layer on legacy kernels (1.5 ms forward + 0.8 ms wgrad of a 22 ms ResNet-50 step).  Here
+cuDNN runs this layer on legacy kernels (C_in = 3 fits no tensor-core tile).  Here
 (``csrc/stem_conv.cu``, ``csrc/gemm_bnstats.cu``):
 
     A  = im2col(x)                    [M, 192] bf16, one 384-byte row per output pixel, k = r*24 + s*3 + c
-    y  = A @ Wp^T  (+ BN statistics)  persistent tcgen05 GEMM; the sums BatchNorm needs come out of its epilogue
+    y  = A @ Wp^T  (+ BN statistics)  persistent wgmma GEMM; the sums BatchNorm needs come out of its epilogue
     -> BN + ReLU + MaxPool            ``stem_forward_pre`` (the statistics pass of the fused stem tail is skipped)
     dW = unpack(dY^T @ A)             library GEMM over the saved A
 
@@ -77,7 +77,7 @@ class _StemConvFn(torch.autograd.Function):
         else:
             from .. import _ext
             C = _ext.lib()
-            _ext.note_launch(2)
+            _ext.note_launch(3)                 # im2col + GEMM + statistics combine
             a = C.stem_im2col(x)
             y = C.conv1x1_bnstats(a, packed.view(packed.size(0), K_PAD, 1, 1), stats)
         ctx.save_for_backward(a, weight)

@@ -7,7 +7,7 @@ Reference call sites (/root/reference/apex_distributed.py):
 
 Semantics kept from apex: O0 fp32 / O1 autocast with fp32 weights / O2 half model + fp32 master weights /
 O3 pure half; dynamic scale starts at 2**16, halves on overflow (and the step is skipped), doubles after 2000 clean
-steps.  B200-native execution: the scale, the growth tracker and the overflow flag live on the device; the
+steps.  H100-native execution: the scale, the growth tracker and the overflow flag live on the device; the
 unscale, the overflow test and the skipped step are folded into the fused optimizer kernel (``csrc/optim.cu``), and
 under a data-parallel engine the non-finite test runs on the *reduced* gradients inside the all-reduce kernel, so
 every rank takes the same decision without any extra collective or host synchronisation.

@@ -26,7 +26,7 @@ from . import plan as P
 KIND_TWO_SHOT, KIND_ONE_SHOT, KIND_BCAST, KIND_PACK, KIND_REDUCE, KIND_PUSH, KIND_UNPACK = range(7)
 FLAG_PREPACKED = 1        # csrc/collectives.cu kPrepacked: gradients already live in the arena (bucket views)
 # payloads up to this size take the one-shot kernel (one barrier, W x the traffic); tools/comm_bench.py measures the crossover
-ONE_SHOT_MAX_BYTES = int(os.environ.get("PTD_ONESHOT_MAX_BYTES", str(512 << 10)))   # 8 x B200: one-shot 35.8 us vs two-shot 36.4 us at 512 KB, 42.3 vs 37.8 at 1 MB
+ONE_SHOT_MAX_BYTES = int(os.environ.get("PTD_ONESHOT_MAX_BYTES", str(512 << 10)))
 _DT = {torch.float32: "fp32", torch.bfloat16: "bf16", torch.float16: "fp16"}
 _TORCH_DT = {"fp32": torch.float32, "bf16": torch.bfloat16, "fp16": torch.float16}
 _VIEW_NAME = {"fp32": "float32", "bf16": "bfloat16", "fp16": "float16"}

@@ -7,7 +7,7 @@ API parity with the reference's use (/root/reference/distributed.py:147-148,223)
 construction, float buffers are re-broadcast from rank 0 before every forward (``broadcast_buffers=True``), buckets
 are 1 MiB (first) / ``bucket_cap_mb`` in reverse registration order, gradients are averaged.
 
-B200-native design:
+H100-native design:
   * the wire format is a symmetric arena mapped into every peer (``parallel/comm.py``); bucket ``k`` owns a fixed
     range of it, so there is no flatten/copy-in: K1 reads the autograd-produced gradients through a pointer pack,
     casts (fp32 -> bf16), pre-scales by 1/world and reduces in ONE kernel per bucket on a high-priority side stream;

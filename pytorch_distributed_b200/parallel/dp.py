@@ -3,7 +3,7 @@
 Call path parity (torch: scatter -> replicate -> parallel_apply -> gather, backward reduce-add onto GPU0):
     model = DataParallel(model, device_ids=gpus, output_device=gpus[0]);  output = model(images);  loss.backward()
 
-B200-native redesign:
+H100-native redesign:
   * **persistent replicas** - ``replicate()``'s per-iteration Python module cloning is gone; each device owns a
     long-lived replica, only the *values* move;
   * **K2' broadcast** - one kernel on the root packs parameters + float buffers into its arena and multicasts them
@@ -174,8 +174,8 @@ class _ReplicaGraph:
 
     Unlike ``torch.cuda.make_graphed_callables`` the parameter gradients never re-enter autograd: the backward graph leaves
     them in ``static_grads`` (fixed addresses), which the K5 pack reads directly - no per-parameter AccumulateGrad, no
-    per-parameter Python at all in the steady state (8 replicas x 161 parameters of ResNet-50 cost the host ~9 ms per step
-    that way, profiles/r2_logs/dp8_host_profile_before.txt).
+    per-parameter Python at all in the steady state (8 replicas x 161 parameters of ResNet-50 cost the host milliseconds per
+    step that way).
     """
 
     def __init__(self, module, params, sample, device, autocast_state):

@@ -7,7 +7,7 @@
     optimizer = hvd.DistributedOptimizer(optimizer, named_parameters=..., compression=hvd.Compression.fp16)  (:159-164)
     hvd.allreduce(tensor, name='barrier')                                        (:104)
 
-Design (B200-native, not a horovod port):
+Design (H100-native, not a horovod port):
   * control plane: ``torch.distributed`` (env:// under torchrun, or the self-spawn launcher) - there is no MPI here;
   * per-parameter hooks enqueue into the C++ :class:`FusionQueue` (``csrc/hvd_core.cpp``); a dispatcher thread pops
     closed fusion groups and launches ONE fused cast(fp32->fp16 "compression") + all-reduce + decompress kernel per

@@ -2,7 +2,7 @@
 
 A *plan* fixes, once, how a list of tensors maps onto a contiguous range of the symmetric arena and how that
 range is cut into per-CTA sub-ranges (``csrc/collectives.cu``: CTA ``b`` owns ``[b*block_elems, (b+1)*block_elems)``
-on every rank).  This is the B200-native counterpart of torch's bucket assignment
+on every rank).  This is the H100-native counterpart of torch's bucket assignment
 (``dist._compute_bucket_assignment_by_size``; reference call site /root/reference/distributed.py:147).
 """
 from __future__ import annotations

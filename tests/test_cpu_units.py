@@ -314,12 +314,26 @@ def test_choose_grid_granularity():
 
 
 def test_reference_install_manifest(tmp_path, monkeypatch):
-    """baseline/install_reference.py: the copy is verified against the sha256 manifest; a tampered file is reported."""
+    """oracle/install_reference.py: the copy is verified against the sha256 manifest; a tampered file is reported."""
+    import hashlib
     import shutil
-    from baseline import install_reference as inst
-    if not os.path.exists("/root/reference/distributed.py"):
-        pytest.skip("reference tree not mounted")
+    from oracle import install_reference as inst
+    src = tmp_path / "reference"                      # a stand-in reference tree with its own manifest
+    src.mkdir()
+    manifest = {}
+    for fn in ("distributed.py", "start.sh"):
+        data = ("# %s\n" % fn).encode()
+        (src / fn).write_bytes(data)
+        manifest[fn] = hashlib.sha256(data).hexdigest()
+    monkeypatch.setattr(inst, "MANIFEST", manifest)
     monkeypatch.setattr(inst, "REF_DIR", str(tmp_path / "_ref"))
+    monkeypatch.setattr(inst, "DEFAULT_DIRS", [str(tmp_path / "absent")])
+    monkeypatch.delenv(inst.ENV, raising=False)
+    assert inst.install(force=True).startswith("NOT INSTALLED")
+    monkeypatch.setattr(inst, "DEFAULT_DIRS", [str(src)])             # found at the default location ...
+    assert inst.install(force=True).startswith("installed") and inst.verify() == []
+    monkeypatch.setattr(inst, "DEFAULT_DIRS", [str(tmp_path / "absent")])
+    monkeypatch.setenv(inst.ENV, str(src))
     msg = inst.install(force=True)
     assert "installed" in msg and inst.verify(str(tmp_path / "_ref")) == []
     with open(tmp_path / "_ref" / "distributed.py", "a") as f:

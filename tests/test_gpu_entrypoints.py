@@ -145,14 +145,14 @@ R50 = ["-a", "resnet50", "-b", "16", "--synthetic", "--steps-per-epoch", "6", "-
 
 
 def test_resnet50_bottleneck_paths_ddp_graph_two_gpus(tmp_path):
-    """ResNet-50 exercises the tcgen05 conv1x1+BN-statistics GEMM inside the captured two-stream step."""
+    """ResNet-50 exercises the wgmma conv1x1+BN-statistics GEMM inside the captured two-stream step."""
     out = _run(_torchrun("distributed.py", 2, R50 + ["--cuda-graph", "--checkpoint-dir", str(tmp_path)], 29806))
     assert out.count(" * Acc@1") == 2
     _finite_losses(out)
 
 
 def test_resnet50_dataparallel_two_gpus(tmp_path):
-    """One process, two devices, replica threads: per-device kernel attributes / TMEM users of the tcgen05 path."""
+    """One process, two devices, replica threads: per-device kernel attributes of the wgmma GEMM path."""
     out = _run([sys.executable, os.path.join(ROOT, "dataparallel.py")] + R50 + ["--gpus", "0,1", "--checkpoint-dir", str(tmp_path)])
     assert out.count(" * Acc@1") == 1
     _finite_losses(out)

@@ -1,5 +1,5 @@
-"""GPU tests of the split-residual-gradient BN backward, the stem im2col + tcgen05 GEMM path and the static horovod schedule
-(written in round 1 without hardware, validated on B200 in round 2 and now the defaults).  Whole-model numerics are judged
+"""GPU tests of the split-residual-gradient BN backward, the stem im2col + wgmma GEMM path and the static horovod schedule
+(all three are the defaults).  Whole-model numerics are judged
 against a plain PyTorch fp32 oracle on a shallow bottleneck ResNet (tests/_oracle.py)."""
 import os
 import sys
@@ -116,7 +116,7 @@ def test_stem_im2col_kernel_matches_definition(shape):
 
 
 def test_stem_gemm_path_matches_cudnn_path():
-    """conv7x7 + BN + ReLU + MaxPool: im2col + tcgen05 GEMM (+ statistics) + stem_forward_pre vs cuDNN conv + fused stem tail."""
+    """conv7x7 + BN + ReLU + MaxPool: im2col + wgmma GEMM (+ statistics) + stem_forward_pre vs cuDNN conv + fused stem tail."""
     import copy
     import torch.nn as nn
     from pytorch_distributed_b200.models.resnet import BNAct

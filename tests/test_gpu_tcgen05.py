@@ -1,4 +1,4 @@
-"""tcgen05 / TMA / TMEM GEMM (1x1 convolution with BatchNorm statistics in the epilogue) against PyTorch fp32."""
+"""wgmma / TMA GEMM (1x1 convolution with BatchNorm statistics in the epilogue) against PyTorch fp32."""
 import copy
 
 import pytest
@@ -52,7 +52,7 @@ def test_bottleneck_with_fused_conv1x1_matches_unfused():
         resnet.FUSED_CONV1X1 = fused
         xx = x.clone().requires_grad_(True)
         begin_step(x.device)
-        y = m(xx)
+        y = resnet._pair(m(xx))[0]     # a training block hands out two aliases of its output (SPLIT_RESGRAD)
         y.float().square().mean().backward()
         outs.append((y.detach().float(), xx.grad.float(), [p.grad.float() for p in m.parameters()], [b.float() for b in m.buffers()]))
     resnet.FUSED_CONV1X1 = False

@@ -1,13 +1,13 @@
 """Micro-benchmarks of the fused collectives (K1..K5) against NCCL and against their link rooflines.
 
-    python -m torch.distributed.run --nproc-per-node 8 --master-addr 127.0.0.1 tools/comm_bench.py [sections...] > profiles/comm_bench_8gpu.md
+    python -m torch.distributed.run --nproc-per-node 8 --master-addr 127.0.0.1 tools/comm_bench.py [sections...] > comm_bench_8gpu.md
     python tools/comm_bench.py local          # single process, all visible GPUs: K2' push / K5 reduce-to-caller (DataParallel engine)
 
 Sections (default: all multi-process ones): k1 k1small ctas k2 k4.
 Every number: device time (CUDA events on the launching stream), max over ranks, median of `reps` after warm-ups, with a
 barrier + synchronize between repetitions.  Rooflines:
-  all-reduce  bus bandwidth 2(W-1)/W * wire_bytes / t   vs the measured 8-rank NCCL reference 725 GB/s (profiling guide)
-  broadcast / push / reduce-to-root   wire_bytes / t     vs the measured 770 GB/s per direction per GPU (root egress or ingress)
+  all-reduce  bus bandwidth 2(W-1)/W * wire_bytes / t   vs 450 GB/s, NVLink 4 per direction per GPU (H100 SXM data sheet)
+  broadcast / push / reduce-to-root   wire_bytes / t     vs the same 450 GB/s per direction per GPU (root egress or ingress)
 """
 import os
 import statistics
@@ -19,7 +19,7 @@ import torch.distributed as dist
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
-BUS_REF, DIR_REF = 725.0, 770.0
+BUS_REF, DIR_REF = 450.0, 450.0
 
 
 def timed(fn, reps, device, sync, reduce_max=True):
@@ -43,7 +43,7 @@ def section_k1(comm_factory, dev, world, sync, say):
     in-arena ("prepacked", gradient_as_bucket_view) variant that has no pack pass at all."""
     from pytorch_distributed_b200.parallel.comm import KIND_TWO_SHOT
     say("\n## K1 two-shot all-reduce (one bucket per launch)\n")
-    say("| wire MB | elements | src->wire | NVLS pack us | NVLS in-arena us | P2P pack us | NCCL us | best busbw GB/s | frac of 725 | in-arena busbw | frac | NCCL busbw |")
+    say("| wire MB | elements | src->wire | NVLS pack us | NVLS in-arena us | P2P pack us | NCCL us | best busbw GB/s | frac of 450 | in-arena busbw | frac | NCCL busbw |")
     say("|---:|---:|---|---:|---:|---:|---:|---:|---:|---:|---:|---:|")
     for n in (1 << 19, 1 << 20, 1 << 21, 1 << 22, 6_000_000, 1 << 23, 1 << 24, 25_600_000, 1 << 26):
         comm = comm_factory()
@@ -127,7 +127,7 @@ def section_k2(comm_factory, dev, world, sync, say):
     bufs = [b for b in model.buffers() if b.is_floating_point()]
     big = [torch.randn(1 << 24, device=dev)]
     say("\n## K2 broadcast from rank 0 (multicast store; root egress = N bytes)\n")
-    say("| tensors | MB | fused us | GB/s (root egress) | frac of 770 | NCCL (flatten + broadcast + unflatten) us |\n|---|---:|---:|---:|---:|---:|")
+    say("| tensors | MB | fused us | GB/s (root egress) | frac of 450 | NCCL (flatten + broadcast + unflatten) us |\n|---|---:|---:|---:|---:|---:|")
     for name, ts_ in (("161 ResNet-50 parameters fp32", params), ("106 BN buffers fp32", bufs), ("1 tensor fp32", big)):
         def fused_b(ts_=ts_):
             comm.broadcast_(ts_, root=0)
@@ -192,7 +192,7 @@ def main_multi(sections):
 
     say = (lambda *a: print(*a, flush=True)) if rank == 0 else (lambda *a: None)
     probe = factory()
-    say("# Fused collectives vs NCCL, %d x B200 (symm=%s, nvls=%s)\n" % (world, probe.symm_backend, probe.nvls))
+    say("# Fused collectives vs NCCL, %d x %s (symm=%s, nvls=%s)\n" % (world, torch.cuda.get_device_name(), probe.symm_backend, probe.nvls))
     say("Device-timed (CUDA events), max over ranks, median of 7 after 3 warm-ups.")
     del probe
     table = {"k1": section_k1, "k1small": section_k1small, "ctas": section_ctas, "k2": section_k2, "k4": section_k4}
@@ -210,9 +210,9 @@ def main_local():
     ndev = torch.cuda.device_count()
     devices = list(range(ndev))
     comm = LocalCommunicator(devices, 1 << 30)
-    print("# Single-process engine kernels over %d x B200 (nvls=%s)\n" % (ndev, comm.nvls))
+    print("# Single-process engine kernels over %d x %s (nvls=%s)\n" % (ndev, torch.cuda.get_device_name(), comm.nvls))
     print("Device time on the ROOT's stream (CUDA events), median of 7 after 3 warm-ups; bf16 values.\n")
-    print("| MB | K2' push us | GB/s | frac of 770 | replica unpack us | K5 pack us | K5 reduce-to-root us | GB/s (root ingress) | frac of 770 |")
+    print("| MB | K2' push us | GB/s | frac of 450 | replica unpack us | K5 pack us | K5 reduce-to-root us | GB/s (root ingress) | frac of 450 |")
     print("|---:|---:|---:|---:|---:|---:|---:|---:|---:|")
     root = torch.device("cuda", 0)
 

@@ -1,4 +1,4 @@
-"""Correctness + speed of the tcgen05 1x1-conv GEMM with fused BN statistics against cuDNN conv + bn_stats."""
+"""Correctness + speed of the wgmma 1x1-conv GEMM with fused BN statistics against cuDNN conv + bn_stats."""
 import sys, os
 import torch
 import torch.nn.functional as F
@@ -53,7 +53,7 @@ for cin, cout, hw in shapes:
             C.bn_act_forward(yy, None, wt, bt, torch.zeros(cout, device="cuda"), torch.ones(cout, device="cuda"), None, True, 0.1, 1e-5, True, False, work, False)
         t_both = t(both)
         tot[0] += t_mine; tot[1] += t_conv; tot[2] += t_both
-        line += " | tcgen05+stats %.1f us, cudnn conv %.1f us, cudnn conv + bn_stats + bn_apply %.1f us" % (t_mine, t_conv, t_both)
+        line += " | gemm+stats %.1f us, cudnn conv %.1f us, cudnn conv + bn_stats + bn_apply %.1f us" % (t_mine, t_conv, t_both)
     print(line, flush=True)
 if len(shapes) > 3:
-    print("sum: tcgen05+stats %.1f us | cudnn conv %.1f us | conv+stats+apply %.1f us" % tuple(tot))
+    print("sum: gemm+stats %.1f us | cudnn conv %.1f us | conv+stats+apply %.1f us" % tuple(tot))

@@ -1,6 +1,6 @@
-"""Stem convolution: cuDNN (fprop / wgrad) vs im2col + tcgen05 GEMM (+BN statistics) + library wgrad, CUDA-event timings.
+"""Stem convolution: cuDNN (fprop / wgrad) vs im2col + wgmma GEMM (+BN statistics) + library wgrad, CUDA-event timings.
 
-    python tools/stem_gemm_probe.py [batch]        # on a B200; prints one markdown table
+    python tools/stem_gemm_probe.py [batch]        # on an H100; prints one markdown table
 """
 import os
 import sys
@@ -61,7 +61,7 @@ def main():
     t = timed(lambda: C.stem_im2col(x))
     print("| im2col kernel | %.0f | %.2f | %.0f |" % (t, gb_a + x.numel() * 2 / 1e9, (gb_a + x.numel() * 2 / 1e9) / t * 1e6))
     t = timed(lambda: C.conv1x1_bnstats(a, wp.view(64, K_PAD, 1, 1), stats))
-    print("| tcgen05 GEMM K=192 N=64 + BN statistics | %.0f | %.2f | %.0f |" % (t, gb_a + gb_y, (gb_a + gb_y) / t * 1e6))
+    print("| wgmma GEMM K=192 N=64 + BN statistics | %.0f | %.2f | %.0f |" % (t, gb_a + gb_y, (gb_a + gb_y) / t * 1e6))
     t = timed(lambda: torch.mm(dy2.t(), rows, out_dtype=torch.float32))
     print("| library wgrad GEMM (dY^T x A), fp32 out | %.0f | %.2f | %.0f |" % (t, gb_a + gb_y, (gb_a + gb_y) / t * 1e6))
     t = timed(lambda: dy2.t() @ rows)
