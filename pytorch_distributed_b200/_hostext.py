@@ -18,7 +18,9 @@ _SRC = os.path.join(_HERE, "csrc", "host", "loader.cpp")
 _NAME = "_L"
 _SO = os.path.join(_HERE, _NAME + ".so")
 _STAMP = os.path.join(_HERE, _NAME + ".hash")
-_FLAGS = ["-O3", "-std=c++17", "-fPIC", "-shared", "-fvisibility=hidden", "-pthread"]
+# -ffp-contract=off: resample() must round every multiply and add on its own, like the device kernel
+# (csrc/resample.cu), also with compilers that contract to FMA by default (GCC on aarch64)
+_FLAGS = ["-O3", "-std=c++17", "-fPIC", "-shared", "-fvisibility=hidden", "-pthread", "-ffp-contract=off"]
 _lock = threading.Lock()
 _mod = None
 

@@ -105,6 +105,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("stem_im2col", &stem_im2col);
   m.def("conv1x1_bnstats", &conv1x1_bnstats);
   m.def("normalize_nhwc", &normalize_nhwc);
+  m.def("resample_normalize", &resample_normalize, py::arg("arena"), py::arg("n"), py::arg("out_h"), py::arg("out_w"), py::arg("max_rows"),
+        py::arg("a"), py::arg("b"), py::arg("out_dtype"), py::arg("channels_last"));
   m.def("p2p_copy_multi", &p2p_copy_multi);
 
   // horovod-style fusion queue (background thread + tensor fusion scheduling), see hvd_core.cpp

@@ -75,4 +75,8 @@ at::Tensor normalize_nhwc(const at::Tensor& src, const at::Tensor& mean, const a
 
 void p2p_copy_multi(std::vector<at::Tensor> src, std::vector<at::Tensor> dst, int64_t run_device);
 
+// ---- resample.cu
+at::Tensor resample_normalize(const at::Tensor& arena, int64_t n, int64_t out_h, int64_t out_w, int64_t max_rows, const at::Tensor& a,
+                              const at::Tensor& b, int64_t out_dtype, bool channels_last);
+
 }  // namespace ptd

@@ -5,7 +5,9 @@
 // (reference distributed.py:160-195, transforms at :165-172 and :183-188).  At thousands of images/s per GPU that host
 // path cannot keep a node busy, so the steady-state loader here is native: no Python, no pickling, no per-sample
 // allocation in the hot loop.  JPEG decoding happens once, offline (tools/make_shards.py).  The device side is the
-// existing fused normalise/cast/NHWC kernel (csrc/data_ops.cu), fed with the uint8 NCHW batches produced here.
+// existing fused normalise/cast/NHWC kernel (csrc/data_ops.cu), fed with the uint8 NCHW batches produced here.  In
+// staging mode (Config::staged) the threads leave the resample to the GPU (csrc/resample.cu) and write, per sample, the
+// source pixels and filter taps it needs instead.
 //
 // Determinism: the epoch permutation and every per-sample random decision are pure functions of
 // (seed, epoch, position in the epoch), so results do not depend on thread scheduling or thread count.
@@ -23,6 +25,7 @@
 #include <condition_variable>
 #include <cstdint>
 #include <cstring>
+#include <memory>
 #include <mutex>
 #include <stdexcept>
 #include <string>
@@ -165,18 +168,28 @@ struct Scratch {
   std::vector<float> rows;       // horizontally resampled rows [n_rows][out_w][3]
 };
 
-// src: HWC uint8 (H x W x 3).  dst: planar CHW uint8 (3 x out_h x out_w).
-void resample(const Record& r, const Box& b, int out_w, int out_h, uint8_t* dst, Scratch& s) {
-  const int W = int(r.w), H = int(r.h);
+// [lo, hi) of the source coordinates the taps read
+std::pair<int, int> tap_span(const Taps& t) {
+  int lo = INT32_MAX, hi = 0;
+  for (size_t o = 0; o < t.first.size(); ++o) {
+    lo = std::min(lo, t.first[o]);
+    hi = std::max(hi, t.first[o] + t.count[o]);
+  }
+  return {lo, hi};
+}
+
+void build_box_taps(Scratch& s, int W, int H, const Box& b, int out_w, int out_h) {
   const int lo_x = b.clamp ? int(b.x0) : 0, hi_x = b.clamp ? int(b.x0 + b.w) : W;
   const int lo_y = b.clamp ? int(b.y0) : 0, hi_y = b.clamp ? int(b.y0 + b.h) : H;
   build_taps(s.tx, out_w, b.x0, b.w, lo_x, std::min(hi_x, W), b.flip);
   build_taps(s.ty, out_h, b.y0, b.h, lo_y, std::min(hi_y, H), false);
-  int y_first = H, y_last = 0;
-  for (int o = 0; o < out_h; ++o) {
-    y_first = std::min(y_first, s.ty.first[o]);
-    y_last = std::max(y_last, s.ty.first[o] + s.ty.count[o]);
-  }
+}
+
+// src: HWC uint8 (H x W x 3).  dst: planar CHW uint8 (3 x out_h x out_w).
+void resample(const Record& r, const Box& b, int out_w, int out_h, uint8_t* dst, Scratch& s) {
+  const int W = int(r.w);
+  build_box_taps(s, W, int(r.h), b, out_w, out_h);
+  const auto [y_first, y_last] = tap_span(s.ty);
   const int n_rows = y_last - y_first;
   s.rows.resize(size_t(n_rows) * out_w * 3);
   const int kx = s.tx.kmax;
@@ -214,6 +227,37 @@ void resample(const Record& r, const Box& b, int out_w, int out_h, uint8_t* dst,
       d0[2 * plane + x] = uint8_t(std::min(255.f, std::max(0.f, a2 + 0.5f)));
     }
   }
+}
+
+// ---------------------------------------------------------------- staging for the device resample
+// In staging mode a worker does not call resample(): it copies the source rectangle the taps read, and the taps, into the
+// slot's arena, and the GPU kernel (csrc/resample.cu) does resample()'s arithmetic.  Slot layout: `batch` StageDesc,
+// then one 16-byte aligned block per sample, placed by a bump pointer: the region (rh x rw x 3 uint8, HWC), then the
+// taps - x first (int32, relative to the region), x count (int32), x weights (float [out_w][kx]), and the same for y.
+struct StageDesc {
+  int64_t region;     // arena offset of the region
+  int64_t taps;       // arena offset of the taps
+  int32_t rw, rh;     // region width and height
+  int32_t kx, ky;     // weights stored per output column / row
+};
+static_assert(sizeof(StageDesc) == 32, "StageDesc layout is mirrored in csrc/resample.cu and tests/test_cpu_device_resample.py");
+
+constexpr size_t kStageAlign = 16;
+size_t align_up(size_t v) { return (v + kStageAlign - 1) & ~(kStageAlign - 1); }
+size_t taps_bytes(int out, int kmax) { return size_t(out) * (2 * sizeof(int32_t) + size_t(kmax) * sizeof(float)); }
+size_t stage_bytes(int rw, int rh, int out_w, int kx, int out_h, int ky) {
+  return align_up(size_t(rw) * rh * 3) + align_up(taps_bytes(out_w, kx) + taps_bytes(out_h, ky));
+}
+size_t table_bytes(int batch) { return align_up(size_t(batch) * sizeof(StageDesc)); }
+int kmax_for(double in_len, int out) { return int(std::ceil(std::max(in_len / out, 1.0))) * 2 + 1; }   // as build_taps
+
+uint8_t* put_taps(uint8_t* p, const Taps& t, int origin) {
+  const size_t out = t.first.size();
+  auto* first = reinterpret_cast<int32_t*>(p);
+  auto* count = first + out;
+  for (size_t o = 0; o < out; ++o) { first[o] = t.first[o] - origin; count[o] = t.count[o]; }
+  std::memcpy(count + out, t.weight.data(), t.weight.size() * sizeof(float));
+  return p + taps_bytes(int(out), t.kmax);
 }
 
 // ---------------------------------------------------------------- shard files
@@ -268,6 +312,7 @@ struct Config {
   int rank, world, threads, depth;
   bool drop_last, shuffle;
   double scale_lo, scale_hi, ratio_lo, ratio_hi, resize_ratio;
+  bool staged;          // stage regions + taps for the device resample instead of resampling on the host
 };
 
 // ---------------------------------------------------------------- the loader
@@ -288,6 +333,20 @@ class ShardLoader {
     if (per_rank_ == 0) throw std::runtime_error("fewer records than ranks with drop_last");
     n_batches_ = c.drop_last ? per_rank_ / c.batch : (per_rank_ + c.batch - 1) / c.batch;
     slot_done_.assign(c.depth, 0);
+    stage_used_.reset(new std::atomic<size_t>[c.depth]);
+    for (int s = 0; s < c.depth; ++s) stage_used_[s].store(0);
+    if (c.staged) {
+      std::vector<std::pair<uint32_t, uint32_t>> shapes;
+      for (const auto& r : records_) shapes.emplace_back(r.w, r.h);
+      std::sort(shapes.begin(), shapes.end());
+      shapes.erase(std::unique(shapes.begin(), shapes.end()), shapes.end());
+      size_t worst = 0;
+      for (const auto& [W, H] : shapes) {
+        worst = std::max(worst, stage_bound(int(W), int(H)));
+        max_rows_ = std::max(max_rows_, rows_bound(int(W), int(H)));
+      }
+      stage_cap_ = table_bytes(c.batch) + size_t(c.batch) * worst;
+    }
   }
 
   ~ShardLoader() { stop(); }
@@ -314,6 +373,7 @@ class ShardLoader {
     consumed_ = 0;
     released_ = 0;
     std::fill(slot_done_.begin(), slot_done_.end(), 0);
+    for (int s = 0; s < cfg_.depth; ++s) stage_used_[s].store(0);
     quit_ = false;
     for (int t = 0; t < cfg_.threads; ++t) workers_.emplace_back([this] { work(); });
   }
@@ -337,6 +397,7 @@ class ShardLoader {
       std::lock_guard<std::mutex> lk(mu_);
       if (released_ >= consumed_) throw std::runtime_error("release() without a matching next()");
       slot_done_[released_ % cfg_.depth] = 0;
+      stage_used_[released_ % cfg_.depth].store(0);
       ++released_;
     }
     cv_free_.notify_all();
@@ -369,7 +430,61 @@ class ShardLoader {
     return out;
   }
 
+  // ---- staging mode
+  size_t stage_capacity() const { return stage_cap_; }      // bytes of one slot's arena
+  int stage_max_rows() const { return max_rows_; }          // most source rows one output row reads, over all records
+  // bytes of the arena in use by the batch next() returned last for `slot`
+  size_t staged_bytes(int slot) const { return table_bytes(cfg_.batch) + stage_used_[slot].load(); }
+
+  // Upper bound of the bytes one sample of a W x H record stages.  Train: the region lies inside the image and the box
+  // is at most W x H (the centred fallback crop included), so kmax is at most that of the whole image.  Val: the box is a
+  // function of (W, H), so the bound is exact; its filter may read outside the box (clamp = false), inside the image.
+  size_t stage_bound(int W, int H) const {
+    if (cfg_.train) return stage_bytes(W, H, cfg_.out_w, kmax_for(W, cfg_.out_w), cfg_.out_h, kmax_for(H, cfg_.out_h));
+    Scratch s;
+    return plan(s, W, H, center_crop(W, H, cfg_.out_w, cfg_.out_h, cfg_.resize_ratio)).bytes;
+  }
+
+  // test hook: bytes staged for sample `pos` of `epoch` if its record is W x H
+  size_t stage_size(int64_t epoch, int64_t pos, int W, int H) const {
+    Scratch s;
+    return plan(s, W, H, box_for(uint64_t(epoch), uint64_t(pos), W, H)).bytes;
+  }
+
  private:
+  struct Plan { int x0, y0, rw, rh; size_t bytes; };
+
+  Plan plan(Scratch& s, int W, int H, const Box& b) const {
+    build_box_taps(s, W, H, b, cfg_.out_w, cfg_.out_h);
+    const auto [x0, x1] = tap_span(s.tx);
+    const auto [y0, y1] = tap_span(s.ty);
+    return {x0, y0, x1 - x0, y1 - y0, stage_bytes(x1 - x0, y1 - y0, cfg_.out_w, s.tx.kmax, cfg_.out_h, s.ty.kmax)};
+  }
+
+  int rows_bound(int W, int H) const {
+    if (cfg_.train) return kmax_for(H, cfg_.out_h);
+    Scratch s;
+    build_box_taps(s, W, H, center_crop(W, H, cfg_.out_w, cfg_.out_h, cfg_.resize_ratio), cfg_.out_w, cfg_.out_h);
+    return s.ty.kmax;
+  }
+
+  // Copy the region and taps of sample i of the batch in `slot` into its arena and write its descriptor.
+  void stage(const Record& r, const Box& b, int slot, size_t i, Scratch& s) {
+    const Plan p = plan(s, int(r.w), int(r.h), b);
+    const size_t table = table_bytes(cfg_.batch);
+    const size_t off = stage_used_[slot].fetch_add(p.bytes);
+    if (off + p.bytes > stage_cap_ - table) throw std::runtime_error("staging arena overflow (bound violated)");
+    uint8_t* arena = reinterpret_cast<uint8_t*>(images_[slot]);
+    uint8_t* region = arena + table + off;
+    const size_t row = size_t(p.rw) * 3;
+    for (int y = 0; y < p.rh; ++y)
+      std::memcpy(region + y * row, r.px + (size_t(p.y0 + y) * r.w + p.x0) * 3, row);
+    uint8_t* taps = region + align_up(row * p.rh);
+    put_taps(put_taps(taps, s.tx, p.x0), s.ty, p.y0);
+    StageDesc d{int64_t(region - arena), int64_t(taps - arena), p.rw, p.rh, s.tx.kmax, s.ty.kmax};
+    std::memcpy(arena + i * sizeof(StageDesc), &d, sizeof d);
+  }
+
   int batch_size_of(size_t k) const {
     const size_t begin = k * cfg_.batch;
     return int(std::min(size_t(cfg_.batch), per_rank_ - begin));
@@ -413,7 +528,8 @@ class ShardLoader {
         const uint32_t rec = order_[item];
         const Record& r = records_[rec];
         const Box b = box_for(epoch_, item, int(r.w), int(r.h));
-        resample(r, b, cfg_.out_w, cfg_.out_h, reinterpret_cast<uint8_t*>(images_[slot]) + i * img_bytes, scratch);
+        if (cfg_.staged) stage(r, b, slot, i, scratch);
+        else resample(r, b, cfg_.out_w, cfg_.out_h, reinterpret_cast<uint8_t*>(images_[slot]) + i * img_bytes, scratch);
         reinterpret_cast<int64_t*>(labels_[slot])[i] = r.label;
         if (!ids_.empty()) reinterpret_cast<int64_t*>(ids_[slot])[i] = int64_t(rec);
         bool complete;
@@ -445,6 +561,9 @@ class ShardLoader {
   std::mutex mu_;
   std::condition_variable cv_done_, cv_free_;
   std::vector<int> slot_done_;
+  std::unique_ptr<std::atomic<size_t>[]> stage_used_;      // per slot: bump pointer of the arena, after the descriptors
+  size_t stage_cap_ = 0;
+  int max_rows_ = 1;
   size_t consumed_ = 0, released_ = 0;
   bool quit_ = false;
   std::string error_;
@@ -468,15 +587,15 @@ PYBIND11_MODULE(_L, m) {
   py::class_<ShardLoader>(m, "ShardLoader")
       .def(py::init([](const std::vector<std::string>& paths, int batch, int out_h, int out_w, bool train, uint64_t seed, int rank,
                        int world, int threads, int depth, bool drop_last, bool shuffle, double scale_lo, double scale_hi,
-                       double ratio_lo, double ratio_hi, double resize_ratio) {
+                       double ratio_lo, double ratio_hi, double resize_ratio, bool staged) {
              Config c{batch, out_h, out_w, train, seed, rank, world, threads, depth, drop_last, shuffle,
-                      scale_lo, scale_hi, ratio_lo, ratio_hi, resize_ratio};
+                      scale_lo, scale_hi, ratio_lo, ratio_hi, resize_ratio, staged};
              return new ShardLoader(paths, c);
            }),
            py::arg("paths"), py::arg("batch"), py::arg("out_h"), py::arg("out_w"), py::arg("train"), py::arg("seed"), py::arg("rank"),
            py::arg("world"), py::arg("threads"), py::arg("depth"), py::arg("drop_last"), py::arg("shuffle"),
            py::arg("scale_lo") = 0.08, py::arg("scale_hi") = 1.0, py::arg("ratio_lo") = 0.75, py::arg("ratio_hi") = 4.0 / 3.0,
-           py::arg("resize_ratio") = 256.0 / 224.0)
+           py::arg("resize_ratio") = 256.0 / 224.0, py::arg("staged") = false)
       .def("size", &ShardLoader::size)
       .def("samples_per_rank", &ShardLoader::samples_per_rank)
       .def("num_batches", &ShardLoader::num_batches)
@@ -487,6 +606,12 @@ PYBIND11_MODULE(_L, m) {
       .def("release", &ShardLoader::release)
       .def("stop", &ShardLoader::stop, py::call_guard<py::gil_scoped_release>())
       .def("crop_params", &ShardLoader::crop_params)
-      .def("epoch_order", &ShardLoader::epoch_order);
+      .def("epoch_order", &ShardLoader::epoch_order)
+      .def("stage_capacity", &ShardLoader::stage_capacity)
+      .def("stage_max_rows", &ShardLoader::stage_max_rows)
+      .def("staged_bytes", &ShardLoader::staged_bytes)
+      .def("stage_bound", &ShardLoader::stage_bound)
+      .def("stage_size", &ShardLoader::stage_size);
+  m.attr("STAGE_DESC_BYTES") = int(sizeof(StageDesc));
   m.def("resample", &resample_once, py::call_guard<py::gil_scoped_release>());
 }

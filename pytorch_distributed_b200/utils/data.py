@@ -14,6 +14,8 @@ from typing import Iterator, Optional, Tuple
 import torch
 import torch.distributed as dist
 
+from .shards import StagedBatch
+
 IMAGENET_MEAN = (0.485, 0.456, 0.406)
 IMAGENET_STD = (0.229, 0.224, 0.225)
 IMAGENET_TRAIN_SIZE = 1281167
@@ -166,19 +168,32 @@ class DataPrefetcher:
             img = img.contiguous(memory_format=torch.channels_last)
         return img
 
+    def _resample(self, staged, arena: torch.Tensor) -> torch.Tensor:
+        """A shard batch staged for the device resample (utils/shards.StagedBatch) -> what _convert gives for the
+        host-resampled uint8 batch, bit for bit."""
+        from .. import _ext
+        code = {torch.float32: 0, torch.bfloat16: 1, torch.float16: 2}[self.dtype]
+        _ext.note_launch()
+        return _ext.lib().resample_normalize(arena, staged.n, staged.out_h, staged.out_w, staged.max_rows, self._a, self._b, code,
+                                             self.channels_last)
+
     def _stage(self, batch):
         img, tgt = batch
-        self.h2d_bytes += img.numel() * img.element_size() + tgt.numel() * tgt.element_size()
+        staged = isinstance(img, StagedBatch)
+        src = img.data if staged else img
+        self.h2d_bytes += src.numel() * src.element_size() + tgt.numel() * tgt.element_size()
         if not self.cuda:
+            if staged:
+                raise RuntimeError("a batch staged for the device resample needs a CUDA prefetcher")
             return self._convert(img), tgt
         with torch.cuda.stream(self.stream):
-            img = img.to(self.device, non_blocking=True)
+            src = src.to(self.device, non_blocking=True)
             tgt = tgt.to(self.device, non_blocking=True)
             if hasattr(self.loader, "batch_copied"):         # ring-buffer loaders recycle the pinned slot after this event
                 ev = torch.cuda.Event()
                 ev.record(self.stream)
                 self.loader.batch_copied(ev)
-            img = self._convert(img)
+            img = self._resample(img, src) if staged else self._convert(src)
         return img, tgt
 
     def next(self):

@@ -6,7 +6,9 @@ production alternative for a node that consumes ~90k images/s: JPEGs are decoded
 (``tools/make_shards.py``), and training reads them through ``csrc/host/loader.cpp`` - mmap, C++ worker threads doing
 RandomResizedCrop + flip (train) or Resize + CenterCrop (val) with an antialiased bilinear filter, output written as
 uint8 NCHW straight into pinned ring slots.  ``DataPrefetcher`` then does the H2D copy and the fused
-normalise / cast / NHWC kernel exactly as for any other uint8 loader.
+normalise / cast / NHWC kernel exactly as for any other uint8 loader.  On a GPU run the threads only stage the source
+pixels and filter taps of each crop (:class:`StagedBatch`) and the resample runs on the GPU (csrc/resample.cu) with
+the same bits as output.
 
 Shard layout (little endian): ``b"PTDSHRD1"``, u32 records, u32 index capacity, ``capacity`` x 24-byte index entries
 ``(u64 offset, u32 height, u32 width, i32 label, u32 channels=3)``, then the raw HWC uint8 pixels.
@@ -151,6 +153,26 @@ class _Sampler:
         self._owner.epoch = int(epoch)
 
 
+class StagedBatch:
+    """A batch staged for resampling on the GPU (``ShardLoader(device_resample=True)``).
+
+    ``data`` is the used prefix of a pinned ring-slot arena: ``n`` 32-byte descriptors, then per sample the source
+    rectangle its filter taps read and the taps themselves (layout: ``StageDesc`` in csrc/host/loader.cpp).
+    ``DataPrefetcher`` copies it to the device and expands it with the ``resample_normalize`` kernel into the tensor
+    ``normalize_nhwc`` makes of the host-resampled ``uint8 [n, 3, out_h, out_w]`` batch, bit for bit.
+    ``max_rows`` bounds the source rows one output row reads (it sizes the kernel's shared memory).
+    """
+
+    __slots__ = ("data", "n", "out_h", "out_w", "max_rows")
+
+    def __init__(self, data: torch.Tensor, n: int, out_h: int, out_w: int, max_rows: int):
+        self.data, self.n, self.out_h, self.out_w, self.max_rows = data, int(n), int(out_h), int(out_w), int(max_rows)
+
+    @property
+    def shape(self) -> Tuple[int, int, int, int]:
+        return (self.n, 3, self.out_h, self.out_w)
+
+
 class ShardLoader:
     """Iterable over ``(uint8 [B,3,H,W], int64 [B])`` batches living in a ring of (pinned) host buffers.
 
@@ -159,6 +181,10 @@ class ShardLoader:
     instead held until that CUDA event has completed.
     ``sampler.set_epoch(e)`` selects the permutation of the next ``iter()``; sharding across ranks follows
     ``DistributedSampler`` (pad by wrapping, rank ``r`` takes positions ``r, r + world, ...``).
+
+    ``device_resample=True`` yields :class:`StagedBatch` instead of the uint8 images: the worker threads only pick the
+    crop box, build the filter taps and copy the source pixels those taps read, and the resample runs on the GPU.
+    Crop boxes, order, labels, ids and the slot protocol are the same as in the default mode.
     """
 
     raw_uint8 = True            # DataPrefetcher must apply the ImageNet mean/std to these pixels
@@ -166,7 +192,8 @@ class ShardLoader:
     def __init__(self, paths: Sequence[str], batch_size: int, image_size: int = 224, train: bool = True, seed: int = 0,
                  rank: int = 0, world: int = 1, workers: int = 4, depth: int = 4, drop_last: bool = False,
                  shuffle: Optional[bool] = None, pin: Optional[bool] = None, with_ids: bool = False,
-                 scale: Tuple[float, float] = (0.08, 1.0), ratio: Tuple[float, float] = (3.0 / 4.0, 4.0 / 3.0)):
+                 scale: Tuple[float, float] = (0.08, 1.0), ratio: Tuple[float, float] = (3.0 / 4.0, 4.0 / 3.0),
+                 device_resample: bool = False):
         from .. import _hostext
         if not paths:
             raise ValueError("no shard files given")
@@ -174,10 +201,14 @@ class ShardLoader:
         self._L = _hostext.lib().ShardLoader(
             list(paths), int(batch_size), int(image_size), int(image_size), bool(train), int(seed) & (2 ** 63 - 1), int(rank),
             int(world), max(1, int(workers)), depth, bool(drop_last), bool(train if shuffle is None else shuffle),
-            float(scale[0]), float(scale[1]), float(ratio[0]), float(ratio[1]), 256.0 / 224.0)
+            float(scale[0]), float(scale[1]), float(ratio[0]), float(ratio[1]), 256.0 / 224.0, bool(device_resample))
         pin = torch.cuda.is_available() if pin is None else pin
-        self.batch_size, self.depth = int(batch_size), depth
-        self._img = [torch.empty((batch_size, 3, image_size, image_size), dtype=torch.uint8, pin_memory=pin) for _ in range(depth)]
+        self.batch_size, self.depth, self.image_size = int(batch_size), depth, int(image_size)
+        self.device_resample = bool(device_resample)
+        if self.device_resample:          # one staging arena per slot, sized for the largest record of these shards
+            self._img = [torch.empty((self._L.stage_capacity(),), dtype=torch.uint8, pin_memory=pin) for _ in range(depth)]
+        else:
+            self._img = [torch.empty((batch_size, 3, image_size, image_size), dtype=torch.uint8, pin_memory=pin) for _ in range(depth)]
         self._tgt = [torch.empty((batch_size,), dtype=torch.int64, pin_memory=pin) for _ in range(depth)]
         self._ids = [torch.empty((batch_size,), dtype=torch.int64) for _ in range(depth)] if with_ids else []
         self._L.set_buffers([t.data_ptr() for t in self._img], [t.data_ptr() for t in self._tgt], [t.data_ptr() for t in self._ids])
@@ -192,6 +223,11 @@ class ShardLoader:
     @property
     def num_records(self) -> int:
         return int(self._L.size())
+
+    @property
+    def staging_bytes(self) -> int:
+        """Pinned bytes of one ring slot's image buffer (the staging arena with ``device_resample``)."""
+        return self._img[0].numel()
 
     def batch_copied(self, event) -> None:
         """The consumer enqueued its copy of the batch it received last; ``event`` completes when that copy is done."""
@@ -228,7 +264,12 @@ class ShardLoader:
                 self._pending.append([None, 0])
                 if self._ids:
                     self.last_ids = self._ids[slot][:n]
-                yield self._img[slot][:n], self._tgt[slot][:n]
+                if self.device_resample:
+                    img = StagedBatch(self._img[slot][:self._L.staged_bytes(slot)], n, self.image_size, self.image_size,
+                                      self._L.stage_max_rows())
+                else:
+                    img = self._img[slot][:n]
+                yield img, self._tgt[slot][:n]
         finally:
             self._L.stop()
 
@@ -243,11 +284,19 @@ def build_shard_loaders(args, batch_size: int, rank: int, world: int):
         raise FileNotFoundError("no train-*.ptds / val-*.ptds under %r (tools/make_shards.py writes them)" % (args.data,))
     seed = args.seed or 0
     workers = max(1, args.workers)
+    # The GPU resample gives the same bits as the host one, so it is used whenever the run is on a GPU;
+    # PTD_DEVICE_RESAMPLE=0 keeps the resample on the host threads (for A/B measurements).
+    on_gpu = (getattr(args, "device", None) or "cuda").startswith("cuda") and torch.cuda.is_available()
+    dev = on_gpu and os.environ.get("PTD_DEVICE_RESAMPLE", "1") != "0"
     # a captured step replays one batch shape: under --cuda-graph the ragged last training batch is dropped (validation is eager)
     drop = bool(getattr(args, "cuda_graph", False))
     train = ShardLoader(train_paths, batch_size, args.image_size, train=True, seed=seed, rank=rank, world=world, workers=workers,
-                        drop_last=drop)
+                        drop_last=drop, device_resample=dev)
     if drop and len(train) == 0:          # fewer samples than one batch: keep them
-        train = ShardLoader(train_paths, batch_size, args.image_size, train=True, seed=seed, rank=rank, world=world, workers=workers)
-    val = ShardLoader(val_paths, batch_size, args.image_size, train=False, seed=seed, rank=rank, world=world, workers=workers)
+        train = ShardLoader(train_paths, batch_size, args.image_size, train=True, seed=seed, rank=rank, world=world, workers=workers,
+                            device_resample=dev)
+    val = ShardLoader(val_paths, batch_size, args.image_size, train=False, seed=seed, rank=rank, world=world, workers=workers,
+                      device_resample=dev)
+    if dev and rank == 0 and not getattr(args, "quiet", False):
+        print("=> shard loader: resampling on the GPU (%d MB pinned staging per train slot)" % (train.staging_bytes >> 20))
     return train, val, train.sampler, val.sampler

@@ -1,7 +1,7 @@
 #!/bin/sh
 # Race / memory checking of the single-GPU kernels (SURVEY section 5 "race detection"): run on a GPU box, e.g.
 #   sh tools/sanitize.sh > sanitize.log 2>&1
-# memcheck: out-of-bounds / misaligned accesses; racecheck: shared-memory hazards (BN combine rows, stem, GEMM staging).
+# memcheck: out-of-bounds / misaligned accesses; racecheck: shared-memory hazards (BN combine rows, stem, GEMM staging, resample bands).
 set -x
 K='bn_act_forward_backward and 256 or fused_sgd_flat_matches or normalize_kernel or metrics_kernel or multi_tensor_scale'
 compute-sanitizer --tool memcheck --error-exitcode 9 python -m pytest tests/test_gpu_kernels.py -q -x -k "$K" -p no:cacheprovider
@@ -12,3 +12,7 @@ compute-sanitizer --tool racecheck --error-exitcode 9 python -m pytest tests/tes
 echo "racecheck(bn) exit $?"
 compute-sanitizer --tool memcheck --error-exitcode 9 python -m pytest tests/test_gpu_tcgen05.py -q -x -k "shape0 or shape1" -p no:cacheprovider
 echo "memcheck(gemm_bnstats) exit $?"
+compute-sanitizer --tool memcheck --error-exitcode 9 python -m pytest tests/test_gpu_data.py -q -x -k "equals_host_resample" -p no:cacheprovider
+echo "memcheck(resample) exit $?"
+compute-sanitizer --tool racecheck --error-exitcode 9 python -m pytest "tests/test_gpu_data.py::test_device_resample_equals_host_resample[True]" -q -x -p no:cacheprovider
+echo "racecheck(resample bands) exit $?"
