@@ -81,26 +81,40 @@ def test_split_residual_gradients_vs_fp32_oracle():
     _variant_vs_oracle(SPLIT_RESGRAD=True)
 
 
-def test_resnet50_full_depth_step_with_both_paths_is_finite():
-    """Full-depth smoke of the split-gradient + stem-GEMM paths (numerics are judged on the shallow model above: a randomly
-    initialised 50-layer net at batch 16 turns the run-to-run noise of the atomically reduced BN statistics into O(10 %)
-    logit differences, so two runs of the SAME path already disagree more than any tolerance worth asserting)."""
+def test_resnet50_full_depth_step_is_bitwise_reproducible():
+    """Two identical full-depth ResNet-50 train steps through the split-gradient + stem-GEMM paths give the same bits:
+    outputs, every gradient and every BN buffer.  The hand-written kernels add their per-CTA partial sums in a fixed
+    order, and cuDNN is held to deterministic algorithms.  (Numerics are judged on the shallow model above.)"""
+    import copy
     import pytorch_distributed_b200.models.resnet as R
     from pytorch_distributed_b200.models import create_model
+    from pytorch_distributed_b200.ops.bn_act import begin_step
     from pytorch_distributed_b200.parallel.amp import cast_model
     torch.manual_seed(0)
     dev = torch.device("cuda", 0)
-    m = cast_model(create_model("resnet50", num_classes=100).to(dev).to(memory_format=torch.channels_last), torch.bfloat16).train()
+    m0 = cast_model(create_model("resnet50", num_classes=100).to(dev).to(memory_format=torch.channels_last), torch.bfloat16).train()
     x = torch.randn(16, 3, 96, 96, device=dev).bfloat16().contiguous(memory_format=torch.channels_last)
     y = torch.randint(0, 100, (16,), device=dev)
+    flags = (torch.backends.cudnn.deterministic, torch.backends.cudnn.benchmark)
+    torch.backends.cudnn.deterministic, torch.backends.cudnn.benchmark = True, False
     R.SPLIT_RESGRAD, R.STEM_GEMM = True, True
+    runs = []
     try:
-        out = m(x)
-        torch.nn.functional.cross_entropy(out.float(), y).backward()
+        for _ in range(2):
+            m = copy.deepcopy(m0)
+            begin_step(dev)
+            out = m(x)
+            torch.nn.functional.cross_entropy(out.float(), y).backward()
+            runs.append((out.detach(), {n: p.grad for n, p in m.named_parameters()}, dict(m.named_buffers())))
     finally:
         R.SPLIT_RESGRAD, R.STEM_GEMM = False, False
+        torch.backends.cudnn.deterministic, torch.backends.cudnn.benchmark = flags
     torch.cuda.synchronize()
-    assert torch.isfinite(out).all() and all(p.grad is not None and torch.isfinite(p.grad).all() for p in m.parameters())
+    (o1, g1, b1), (o2, g2, b2) = runs
+    assert torch.isfinite(o1).all() and all(g is not None and torch.isfinite(g).all() for g in g1.values())
+    assert torch.equal(o1, o2)
+    assert [n for n in g1 if not torch.equal(g1[n], g2[n])] == []
+    assert [n for n in b1 if not torch.equal(b1[n], b2[n])] == []
 
 
 @pytest.mark.parametrize("shape", [(4, 3, 64, 64), (2, 3, 75, 91), (16, 3, 224, 224)])

@@ -12,6 +12,10 @@ compute-sanitizer --tool racecheck --error-exitcode 9 python -m pytest tests/tes
 echo "racecheck(bn) exit $?"
 compute-sanitizer --tool memcheck --error-exitcode 9 python -m pytest tests/test_gpu_tcgen05.py -q -x -k "shape0 or shape1" -p no:cacheprovider
 echo "memcheck(gemm_bnstats) exit $?"
+compute-sanitizer --tool memcheck --error-exitcode 9 python -m pytest tests/test_gpu_fp64.py -q -x -k "one_cta_second_tile_n64" -p no:cacheprovider
+echo "memcheck(gemm_bnstats, a CTA's second m-tile) exit $?"
+compute-sanitizer --tool racecheck --error-exitcode 9 python -m pytest tests/test_gpu_fp64.py -q -x -k "rpb3_odd_13x14_fp16_c32" -p no:cacheprovider
+echo "racecheck(stem backward, quad rows crossing images) exit $?"
 compute-sanitizer --tool memcheck --error-exitcode 9 python -m pytest tests/test_gpu_data.py -q -x -k "equals_host_resample" -p no:cacheprovider
 echo "memcheck(resample) exit $?"
 compute-sanitizer --tool racecheck --error-exitcode 9 python -m pytest "tests/test_gpu_data.py::test_device_resample_equals_host_resample[True]" -q -x -p no:cacheprovider
