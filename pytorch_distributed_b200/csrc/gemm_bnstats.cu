@@ -1,7 +1,7 @@
 // 1x1 convolution (NHWC) as a wgmma GEMM with the BatchNorm statistics fused into the epilogue (sm_90a).
 //
-//   C[M, N] (bf16) = A[M, K] (bf16 activations, K = C_in contiguous) x B[N, K]^T (bf16 weights [C_out, C_in])
-//   gsum[0:N]  += sum_m C[m, n]          gsum[N:2N] += sum_m C[m, n]^2          (fp32, over the stored bf16 values)
+//   C[M, N] (T) = A[M, K] (T activations, K = C_in contiguous) x B[N, K]^T (T weights [C_out, C_in]),  T = bf16 or fp16
+//   gsum[0:N]  += sum_m C[m, n]          gsum[N:2N] += sum_m C[m, n]^2          (fp32, over the stored 16-bit values)
 //
 // In a ResNet-50 step the 1x1 convolutions are HBM-bound, so the only way to make them cheaper is to do more per byte:
 // the per-channel sum / sum-of-squares that BatchNorm needs are reduced here from the output tile while it sits in
@@ -15,9 +15,15 @@
 //   warp 8        TMA producer : cp.async.bulk.tensor.2d (128B-swizzled 128x64 A tile, BLOCK_Nx64 B tile) -> smem ring,
 //                                completion on an mbarrier (expect_tx); runs ahead across tile boundaries
 //   warpgroups 0,1 consumers   : warpgroup c owns rows [64c, 64c+64) of the 128-row tile; wgmma.mma_async m64nXk16
-//                                (bf16 x bf16 -> fp32 registers) straight from the swizzled smem stages; epilogue packs
-//                                bf16 into a 128B-swizzled staging tile, one TMA store per 64x64 box (clipped at the M
+//                                (T x T -> fp32 registers) straight from the swizzled smem stages; epilogue packs
+//                                T into a 128B-swizzled staging tile, one TMA store per 64x64 box (clipped at the M
 //                                tail by the tensor map), column owners reduce the statistics from the staged values.
+//
+// bf16 and fp16 share everything but the wgmma operand type, the tensor-map element type and the pack / unpack of the
+// epilogue (both are 2-byte elements with the same swizzled layout).  Products of two fp16 (or two bf16) values are exact
+// in fp32, so both accumulate the same way.  fp16 output is rounded to nearest even (__floats2half2_rn): a value of
+// magnitude >= 65520 is stored as +-inf, and the sums of that channel become inf / nan - what cuDNN followed by a separate
+// statistics pass over the stored tensor gives.
 #include <ATen/cuda/CUDAContext.h>
 #include <c10/cuda/CUDAGuard.h>
 #include <cuda.h>
@@ -29,7 +35,7 @@
 namespace ptd {
 
 constexpr int kBlockM = 128;
-constexpr int kBlockK = 64;          // 64 bf16 = one 128-byte swizzle row
+constexpr int kBlockK = 64;          // 64 16-bit elements = one 128-byte swizzle row
 constexpr int kConsumerThreads = 256;
 constexpr int kGemmThreads = kConsumerThreads + 32;
 
@@ -37,7 +43,7 @@ template <int BLOCK_N> struct GemmCfg {
   static constexpr int kStages = BLOCK_N == 256 ? 3 : 4;
   static constexpr int kABytes = kBlockM * kBlockK * 2;
   static constexpr int kBBytes = BLOCK_N * kBlockK * 2;
-  static constexpr int kCBytes = kBlockM * BLOCK_N * 2;               // bf16 output staging, [BLOCK_N / 64] 64-column boxes
+  static constexpr int kCBytes = kBlockM * BLOCK_N * 2;               // 16-bit output staging, [BLOCK_N / 64] 64-column boxes
   static constexpr int kStatFloats = 2 * 4 * 128;                     // [2 warpgroups][4 sums][128 threads]
   static constexpr int kSmem = 1024 + kStages * (kABytes + kBBytes) + kCBytes + kStatFloats * 4 + 2 * kStages * 8;
 };
@@ -72,7 +78,7 @@ __device__ __forceinline__ void named_barrier(int id, int threads) {
 }
 
 // wgmma shared-memory matrix descriptor: K-major, 128-byte swizzle, 8-row groups 1024 bytes apart (SBO), LBO unused (=1).
-// The tile is 1024-byte aligned; +2 in the (>>4) start-address field advances K by 16 bf16 (32 bytes).
+// The tile is 1024-byte aligned; +2 in the (>>4) start-address field advances K by 16 elements (32 bytes).
 __device__ __forceinline__ uint64_t gmma_desc(const void* smem_tile) {
   const uint64_t addr = (uint64_t)(smem_u32(smem_tile) >> 4) & 0x3FFFull;
   return addr | (1ull << 16) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 62);
@@ -80,28 +86,37 @@ __device__ __forceinline__ uint64_t gmma_desc(const void* smem_tile) {
 
 #define PTD_F8(i) "+f"(d[i]), "+f"(d[i + 1]), "+f"(d[i + 2]), "+f"(d[i + 3]), "+f"(d[i + 4]), "+f"(d[i + 5]), "+f"(d[i + 6]), "+f"(d[i + 7])
 
-// D[64 x 64] (+)= A[64 x 16] * B[64 x 16]^T, fp32 accumulators in d[32]
-__device__ __forceinline__ void wgmma_n64(float* d, uint64_t adesc, uint64_t bdesc, int accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n\t}"
-      : PTD_F8(0), PTD_F8(8), PTD_F8(16), PTD_F8(24)
-      : "l"(adesc), "l"(bdesc), "r"(accumulate));
-}
+// D[64 x 64] (+)= A[64 x 16] * B[64 x 16]^T, fp32 accumulators in d[32]; TY: the operand type, "bf16" or "f16"
+#define PTD_WGMMA_N64(TY)                                                                                             \
+  asm volatile(                                                                                                       \
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"                                                              \
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32." TY "." TY " "                                                     \
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "                                       \
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n\t}" \
+      : PTD_F8(0), PTD_F8(8), PTD_F8(16), PTD_F8(24)                                                                  \
+      : "l"(adesc), "l"(bdesc), "r"(accumulate))
 // D[64 x 128] (+)= A[64 x 16] * B[128 x 16]^T, fp32 accumulators in d[64]
-__device__ __forceinline__ void wgmma_n128(float* d, uint64_t adesc, uint64_t bdesc, int accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
-      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
-      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n\t}"
-      : PTD_F8(0), PTD_F8(8), PTD_F8(16), PTD_F8(24), PTD_F8(32), PTD_F8(40), PTD_F8(48), PTD_F8(56)
-      : "l"(adesc), "l"(bdesc), "r"(accumulate));
+#define PTD_WGMMA_N128(TY)                                                                                            \
+  asm volatile(                                                                                                       \
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"                                                              \
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32." TY "." TY " "                                                    \
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "                                       \
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "                              \
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "                              \
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n\t}" \
+      : PTD_F8(0), PTD_F8(8), PTD_F8(16), PTD_F8(24), PTD_F8(32), PTD_F8(40), PTD_F8(48), PTD_F8(56)                  \
+      : "l"(adesc), "l"(bdesc), "r"(accumulate))
+
+template <typename T> __device__ __forceinline__ void wgmma_n64(float* d, uint64_t adesc, uint64_t bdesc, int accumulate) {
+  if constexpr (std::is_same<T, __half>::value) PTD_WGMMA_N64("f16");
+  else PTD_WGMMA_N64("bf16");
 }
+template <typename T> __device__ __forceinline__ void wgmma_n128(float* d, uint64_t adesc, uint64_t bdesc, int accumulate) {
+  if constexpr (std::is_same<T, __half>::value) PTD_WGMMA_N128("f16");
+  else PTD_WGMMA_N128("bf16");
+}
+#undef PTD_WGMMA_N64
+#undef PTD_WGMMA_N128
 #undef PTD_F8
 
 // keeps the compiler from moving accumulator reads / writes across the asynchronous wgmma window
@@ -110,7 +125,7 @@ template <int N> __device__ __forceinline__ void fence_regs(float (&d)[N]) {
   for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-template <int BLOCK_N>
+template <typename T, int BLOCK_N>
 __global__ void __launch_bounds__(kGemmThreads, 1) gemm_bnstats_kernel(const __grid_constant__ CUtensorMap tmap_a,
                                                                        const __grid_constant__ CUtensorMap tmap_b,
                                                                        const __grid_constant__ CUtensorMap tmap_c,
@@ -122,9 +137,9 @@ __global__ void __launch_bounds__(kGemmThreads, 1) gemm_bnstats_kernel(const __g
   constexpr int kBoxes = BLOCK_N / 64;                               // 64-column output boxes
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  uint8_t* smem_a = smem;                                            // [kStages][128 x 64] bf16, 128B swizzle
+  uint8_t* smem_a = smem;                                            // [kStages][128 x 64] T, 128B swizzle
   uint8_t* smem_b = smem_a + kStages * Cfg::kABytes;                 // [kStages][BLOCK_N x 64]
-  uint8_t* smem_c = smem_b + kStages * Cfg::kBBytes;                 // [2 warpgroups][kBoxes][64 x 64] bf16, 128B swizzle
+  uint8_t* smem_c = smem_b + kStages * Cfg::kBBytes;                 // [2 warpgroups][kBoxes][64 x 64] T, 128B swizzle
   float* smem_stats = reinterpret_cast<float*>(smem_c + Cfg::kCBytes);   // [2 warpgroups][s0 s1 q0 q1][128 threads]
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem_stats + Cfg::kStatFloats);
   uint64_t* empty_bar = full_bar + kStages;
@@ -187,8 +202,8 @@ __global__ void __launch_bounds__(kGemmThreads, 1) gemm_bnstats_kernel(const __g
 #pragma unroll
         for (int h = 0; h < BLOCK_N / kInstN; ++h) {
           // B rows [h * kInstN, ...) start h * kInstN * 128 bytes further: +8 * kInstN in the (>>4) address field
-          if constexpr (kInstN == 128) wgmma_n128(acc + h * 64, adesc + 2 * k, bdesc + h * 8 * kInstN + 2 * k, (kb | k) != 0);
-          else wgmma_n64(acc + h * 32, adesc + 2 * k, bdesc + h * 8 * kInstN + 2 * k, (kb | k) != 0);
+          if constexpr (kInstN == 128) wgmma_n128<T>(acc + h * 64, adesc + 2 * k, bdesc + h * 8 * kInstN + 2 * k, (kb | k) != 0);
+          else wgmma_n64<T>(acc + h * 32, adesc + 2 * k, bdesc + h * 8 * kInstN + 2 * k, (kb | k) != 0);
         }
       }
       asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
@@ -205,9 +220,9 @@ __global__ void __launch_bounds__(kGemmThreads, 1) gemm_bnstats_kernel(const __g
       // 16-byte granule g of row r sits at slot g ^ (r & 7) (the TMA SWIZZLE_128B layout): conflict-free here and below
       uint8_t* box = stg + (j >> 3) * 8192 + (lane & 3) * 4;
       const int g = j & 7;
-      *reinterpret_cast<uint32_t*>(box + r0 * 128 + ((g ^ (r0 & 7)) << 4)) = Wire<__nv_bfloat16>::pack2(acc[4 * j], acc[4 * j + 1]);
+      *reinterpret_cast<uint32_t*>(box + r0 * 128 + ((g ^ (r0 & 7)) << 4)) = Wire<T>::pack2(acc[4 * j], acc[4 * j + 1]);
       *reinterpret_cast<uint32_t*>(box + (r0 + 8) * 128 + ((g ^ (r0 & 7)) << 4)) =
-          Wire<__nv_bfloat16>::pack2(acc[4 * j + 2], acc[4 * j + 3]);
+          Wire<T>::pack2(acc[4 * j + 2], acc[4 * j + 3]);
     }
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");     // generic-proxy writes -> visible to the TMA engine
     named_barrier(1 + wg, 128);
@@ -218,12 +233,12 @@ __global__ void __launch_bounds__(kGemmThreads, 1) gemm_bnstats_kernel(const __g
                      ::"l"(&tmap_c), "r"(smem_u32(stg + b * 8192)), "r"(n0 + b * 64), "r"(mt * kBlockM + wg * 64) : "memory");
       asm volatile("cp.async.bulk.commit_group;" ::: "memory");
     }
-    // The statistics are taken from the bf16-rounded values - exactly what a separate BatchNorm pass over the stored
+    // The statistics are taken from the rounded 16-bit values - exactly what a separate BatchNorm pass over the stored
     // tensor would see.  Rows past M were zero-filled by TMA: they contribute 0 to both sums.
     const uint8_t* src = stg + p_box * 8192 + p_byte;
 #pragma unroll 8
     for (int r = rpart * kRows; r < rpart * kRows + kRows; ++r) {
-      const float2 f = Wire<__nv_bfloat16>::unpack2(*reinterpret_cast<const uint32_t*>(src + r * 128 + ((p_gran ^ (r & 7)) << 4)));
+      const float2 f = Wire<T>::unpack2(*reinterpret_cast<const uint32_t*>(src + r * 128 + ((p_gran ^ (r & 7)) << 4)));
       s0 += f.x; q0 += f.x * f.x;
       s1 += f.y; q1 += f.y * f.y;
     }
@@ -260,48 +275,60 @@ static EncodeTiledFn encode_fn() {
   return fn;
 }
 
-// row-major [rows, cols] bf16 matrix, box = box_rows x 64 columns, 128-byte swizzle
-static CUtensorMap make_map(const void* ptr, int64_t rows, int64_t cols, int box_rows, CUtensorMapL2promotion promo) {
+// row-major [rows, cols] matrix of 16-bit elements (dtype: BFLOAT16 / FLOAT16), box = box_rows x 64 columns, 128-byte swizzle
+static CUtensorMap make_map(CUtensorMapDataType dtype, const void* ptr, int64_t rows, int64_t cols, int box_rows,
+                            CUtensorMapL2promotion promo) {
   CUtensorMap m;
   cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
   cuuint64_t strides[1] = {(cuuint64_t)cols * 2};
   cuuint32_t box[2] = {(cuuint32_t)kBlockK, (cuuint32_t)box_rows};
   cuuint32_t estr[2] = {1, 1};
-  CUresult r = encode_fn()(&m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(ptr), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+  CUresult r = encode_fn()(&m, dtype, 2, const_cast<void*>(ptr), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                            CU_TENSOR_MAP_SWIZZLE_128B, promo, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   TORCH_CHECK(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled failed: ", (int)r);
   return m;
 }
 
-template <int BLOCK_N>
+template <typename T, int BLOCK_N>
 static void launch_gemm(const at::Tensor& a, const at::Tensor& b, at::Tensor& c, at::Tensor& gsum, int M, int N, int K) {
   constexpr int smem = GemmCfg<BLOCK_N>::kSmem;
   static bool configured[64] = {};                 // the attribute is per device (DataParallel drives several from one process)
   const int dev = a.get_device();
   if (!configured[dev & 63]) {
-    C10_CUDA_CHECK(cudaFuncSetAttribute(gemm_bnstats_kernel<BLOCK_N>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    C10_CUDA_CHECK(cudaFuncSetAttribute(gemm_bnstats_kernel<T, BLOCK_N>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     configured[dev & 63] = true;
   }
-  const CUtensorMap ma = make_map(a.data_ptr(), M, K, kBlockM, CU_TENSOR_MAP_L2_PROMOTION_L2_256B);
-  const CUtensorMap mb = make_map(b.data_ptr(), N, K, BLOCK_N, CU_TENSOR_MAP_L2_PROMOTION_L2_256B);
-  const CUtensorMap mc = make_map(c.data_ptr(), M, N, 64, CU_TENSOR_MAP_L2_PROMOTION_NONE);   // 64 x 64 store boxes
+  constexpr CUtensorMapDataType dt = std::is_same<T, __half>::value ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
+  const CUtensorMap ma = make_map(dt, a.data_ptr(), M, K, kBlockM, CU_TENSOR_MAP_L2_PROMOTION_L2_256B);
+  const CUtensorMap mb = make_map(dt, b.data_ptr(), N, K, BLOCK_N, CU_TENSOR_MAP_L2_PROMOTION_L2_256B);
+  const CUtensorMap mc = make_map(dt, c.data_ptr(), M, N, 64, CU_TENSOR_MAP_L2_PROMOTION_NONE);   // 64 x 64 store boxes
   const int m_tiles = (M + kBlockM - 1) / kBlockM, n_tiles = N / BLOCK_N;
   const int sms = at::cuda::getCurrentDeviceProperties()->multiProcessorCount;
   const int ctas_per_n = std::max(1, std::min(m_tiles, sms / n_tiles));
   const int grid = ctas_per_n * n_tiles;
   cudaStream_t st = at::cuda::getCurrentCUDAStream();
   at::Tensor part = at::empty({ctas_per_n, 2 * N}, gsum.options());
-  gemm_bnstats_kernel<BLOCK_N><<<grid, kGemmThreads, smem, st>>>(ma, mb, mc, part.data_ptr<float>(), N, K, m_tiles, n_tiles, ctas_per_n);
+  gemm_bnstats_kernel<T, BLOCK_N><<<grid, kGemmThreads, smem, st>>>(ma, mb, mc, part.data_ptr<float>(), N, K, m_tiles, n_tiles, ctas_per_n);
   C10_CUDA_KERNEL_LAUNCH_CHECK();
   combine_partials(part.data_ptr<float>(), ctas_per_n, 2 * N, gsum.data_ptr<float>(), st);
 }
 
-// x: [B, K, H, W] channels_last bf16; weight: [N, K, 1, 1] bf16 (any dense layout); gsum: zeroed float[2N].
-// returns y [B, N, H, W] channels_last bf16; gsum accumulates the per-channel sum and sum of squares of y.
+template <typename T>
+static void launch_gemm_for(const at::Tensor& a, const at::Tensor& b, at::Tensor& c, at::Tensor& gsum, int M, int N, int K) {
+  static const int max_bn = getenv("PTD_GEMM_BLOCK_N") ? atoi(getenv("PTD_GEMM_BLOCK_N")) : 256;
+  if (N % 256 == 0 && max_bn >= 256) launch_gemm<T, 256>(a, b, c, gsum, M, N, K);
+  else if (N % 128 == 0 && max_bn >= 128) launch_gemm<T, 128>(a, b, c, gsum, M, N, K);
+  else launch_gemm<T, 64>(a, b, c, gsum, M, N, K);
+}
+
+// x: [B, K, H, W] channels_last bf16 or fp16; weight: [N, K, 1, 1] of x's dtype (any dense layout); gsum: zeroed float[2N].
+// returns y [B, N, H, W] channels_last in x's dtype; gsum accumulates the per-channel sum and sum of squares of y.
 at::Tensor conv1x1_bnstats(const at::Tensor& x, const at::Tensor& weight, at::Tensor gsum) {
-  TORCH_CHECK(x.is_cuda() && x.dim() == 4 && x.scalar_type() == at::kBFloat16 && x.is_contiguous(at::MemoryFormat::ChannelsLast),
-              "conv1x1_bnstats: x must be a channels_last bf16 CUDA tensor");
-  TORCH_CHECK(weight.dim() == 4 && weight.size(2) == 1 && weight.size(3) == 1 && weight.scalar_type() == at::kBFloat16, "weight must be [N, K, 1, 1] bf16");
+  const bool is16 = x.scalar_type() == at::kBFloat16 || x.scalar_type() == at::kHalf;
+  TORCH_CHECK(x.is_cuda() && x.dim() == 4 && is16 && x.is_contiguous(at::MemoryFormat::ChannelsLast),
+              "conv1x1_bnstats: x must be a channels_last bf16 or fp16 CUDA tensor");
+  TORCH_CHECK(weight.dim() == 4 && weight.size(2) == 1 && weight.size(3) == 1 && weight.scalar_type() == x.scalar_type(),
+              "conv1x1_bnstats: weight must be [N, K, 1, 1] with x's dtype (both bf16 or both fp16)");
   const int64_t M64 = x.size(0) * x.size(2) * x.size(3);
   const int K = (int)x.size(1), N = (int)weight.size(0);
   TORCH_CHECK(weight.size(1) == K && K % kBlockK == 0 && N % 64 == 0 && M64 < (int64_t)1 << 31, "conv1x1_bnstats: unsupported shape");
@@ -311,10 +338,8 @@ at::Tensor conv1x1_bnstats(const at::Tensor& x, const at::Tensor& weight, at::Te
   at::Tensor w2 = weight.reshape({N, K}).contiguous();       // [N, K] K-major (a view for both NCHW and NHWC 1x1 weights)
   at::Tensor y = at::empty({x.size(0), N, x.size(2), x.size(3)}, x.options().memory_format(at::MemoryFormat::ChannelsLast));
   const int M = (int)M64;
-  static const int max_bn = getenv("PTD_GEMM_BLOCK_N") ? atoi(getenv("PTD_GEMM_BLOCK_N")) : 256;
-  if (N % 256 == 0 && max_bn >= 256) launch_gemm<256>(x, w2, y, gsum, M, N, K);
-  else if (N % 128 == 0 && max_bn >= 128) launch_gemm<128>(x, w2, y, gsum, M, N, K);
-  else launch_gemm<64>(x, w2, y, gsum, M, N, K);
+  if (x.scalar_type() == at::kHalf) launch_gemm_for<__half>(x, w2, y, gsum, M, N, K);
+  else launch_gemm_for<__nv_bfloat16>(x, w2, y, gsum, M, N, K);
   return y;
 }
 

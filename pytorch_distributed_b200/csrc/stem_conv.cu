@@ -8,6 +8,7 @@
 // K ordering of a row: k = r*24 + s*3 + c for filter row r < 7, filter column s < 7, channel c < 3; positions with
 // s*3 + c >= 21 and k >= 168 are zero (the packed weights are zero there too).  A filter row is 21 CONTIGUOUS input
 // elements in NHWC, so a 16-byte granule of A is 8 consecutive input elements: one thread builds one granule.
+// im2col only moves 16-bit values, so one pair of kernels serves bf16 and fp16 (A has the input's dtype).
 // Reference call site: torchvision resnet.conv1 reached through /root/reference/distributed.py:136-139.
 #include <ATen/cuda/CUDAContext.h>
 #include <c10/cuda/CUDAGuard.h>
@@ -36,7 +37,7 @@ __device__ __forceinline__ V4 stem_granule_scalar(const unsigned short* __restri
 }
 
 // Fallback (odd row lengths / unaligned base): one granule per thread straight from global memory.
-__global__ void __launch_bounds__(256) stem_im2col_scalar_kernel(const __nv_bfloat16* __restrict__ x, __nv_bfloat16* __restrict__ a, int H,
+__global__ void __launch_bounds__(256) stem_im2col_scalar_kernel(const unsigned short* __restrict__ x, unsigned short* __restrict__ a, int H,
                                                                  int W, int OH, int OW) {
   const int g = blockIdx.y * blockDim.x + threadIdx.x;       // granule inside the output row
   if (g >= OW * kStemGranules) return;
@@ -48,7 +49,7 @@ __global__ void __launch_bounds__(256) stem_im2col_scalar_kernel(const __nv_bflo
   V4 o{0u, 0u, 0u, 0u};
   const int ih = 2 * oh - 3 + r;
   if (r < 7 && ih >= 0 && ih < H) {
-    const unsigned short* row = reinterpret_cast<const unsigned short*>(x) + ((int64_t)n * H + ih) * row_elems;
+    const unsigned short* row = x + ((int64_t)n * H + ih) * row_elems;
     o = stem_granule_scalar(row, (2 * ow - 3) * 3 + q * 8, q, row_elems);
   }
   st_v4(a + ((int64_t)orow * OW * kStemGranules + g) * 8, o);
@@ -61,7 +62,7 @@ __global__ void __launch_bounds__(256) stem_im2col_scalar_kernel(const __nv_bflo
 // 4-byte word - so a granule is five aligned 32-bit shared loads and four PRMTs (hi half of word k | lo half of word k+1).
 constexpr int kStemPad = 16;          // zero elements before / after each staged row (multiple of 8: keeps 16-byte alignment)
 
-__global__ void __launch_bounds__(256) stem_im2col_kernel(const __nv_bfloat16* __restrict__ x, __nv_bfloat16* __restrict__ a, int H, int W,
+__global__ void __launch_bounds__(256) stem_im2col_kernel(const unsigned short* __restrict__ x, unsigned short* __restrict__ a, int H, int W,
                                                           int OH, int OW) {
   extern __shared__ __align__(16) unsigned char stem_smem[];
   const int row_elems = W * 3;                               // host guarantees row_elems % 8 == 0 (16-byte rows)
@@ -76,12 +77,12 @@ __global__ void __launch_bounds__(256) stem_im2col_kernel(const __nv_bfloat16* _
     const int e = c * 8 - kStemPad;                          // first input element of this vector
     V4 val{0u, 0u, 0u, 0u};
     if (ih >= 0 && ih < H && e >= 0 && e < row_elems)
-      val = ld_stream(reinterpret_cast<const unsigned short*>(x) + ((int64_t)n * H + ih) * row_elems + e);
+      val = ld_stream(x + ((int64_t)n * H + ih) * row_elems + e);
     *reinterpret_cast<V4*>(sm + r * srow + c * 8) = val;
   }
   __syncthreads();
   const int total = OW * kStemGranules;
-  __nv_bfloat16* out = a + (int64_t)orow * total * 8;
+  unsigned short* out = a + (int64_t)orow * total * 8;
   for (int g = threadIdx.x; g < total; g += blockDim.x) {
     const int ow = g / kStemGranules, gq = g - ow * kStemGranules;
     const int r = gq / 3, q = gq - 3 * r;                    // filter row, granule inside the row (r == 7: zero padding of K)
@@ -103,12 +104,12 @@ __global__ void __launch_bounds__(256) stem_im2col_kernel(const __nv_bfloat16* _
   }
 }
 
-// x: [N, 3, H, W] channels_last bf16 (physically N x H x W x 3).  returns A as a [N, 192, OH, OW] channels_last view
-// (physically [N*OH*OW, 192] row-major), which is exactly the activation layout conv1x1_bnstats() takes.
+// x: [N, 3, H, W] channels_last bf16 or fp16 (physically N x H x W x 3).  returns A (x's dtype) as a [N, 192, OH, OW]
+// channels_last view (physically [N*OH*OW, 192] row-major), which is exactly the activation layout conv1x1_bnstats() takes.
 at::Tensor stem_im2col(const at::Tensor& x) {
-  TORCH_CHECK(x.is_cuda() && x.dim() == 4 && x.size(1) == 3 && x.scalar_type() == at::kBFloat16 &&
+  TORCH_CHECK(x.is_cuda() && x.dim() == 4 && x.size(1) == 3 && (x.scalar_type() == at::kBFloat16 || x.scalar_type() == at::kHalf) &&
                   x.is_contiguous(at::MemoryFormat::ChannelsLast),
-              "stem_im2col: x must be a [N, 3, H, W] channels_last bf16 CUDA tensor");
+              "stem_im2col: x must be a [N, 3, H, W] channels_last bf16 or fp16 CUDA tensor");
   const int64_t N = x.size(0);
   const int H = (int)x.size(2), W = (int)x.size(3);
   const int OH = (H + 6 - 7) / 2 + 1, OW = (W + 6 - 7) / 2 + 1;
@@ -116,8 +117,8 @@ at::Tensor stem_im2col(const at::Tensor& x) {
   c10::cuda::CUDAGuard guard(x.device());
   at::Tensor a = at::empty({N, OH, OW, kStemK}, x.options());
   TORCH_CHECK(N * OH < ((int64_t)1 << 31) && (int64_t)OW * kStemGranules < (1 << 24), "stem_im2col: too many output rows");
-  const __nv_bfloat16* xp = reinterpret_cast<const __nv_bfloat16*>(x.data_ptr());
-  __nv_bfloat16* ap = reinterpret_cast<__nv_bfloat16*>(a.data_ptr());
+  const unsigned short* xp = reinterpret_cast<const unsigned short*>(x.data_ptr());
+  unsigned short* ap = reinterpret_cast<unsigned short*>(a.data_ptr());
   cudaStream_t st = at::cuda::getCurrentCUDAStream();
   const int64_t row_elems = (int64_t)W * 3;
   const size_t smem = (size_t)7 * (row_elems + 2 * kStemPad) * 2;

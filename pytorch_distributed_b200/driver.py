@@ -411,7 +411,7 @@ class HorovodStrategy(Strategy):
     """/root/reference/horovod_distributed.py: broadcast_parameters + DistributedOptimizer(compression=fp16)."""
     name = "horovod_distributed"
     overlap_optimizer = False   # horovod semantics: step() synchronises the handles first, then updates
-    cast_params = True          # bf16 model (wgmma conv / stem GEMM paths need bf16 weights); fp32 masters live in FusedSGD
+    cast_params = True          # 16-bit model, fp32 masters in FusedSGD (fp32 weights + autocast take the same wgmma conv / stem GEMM paths)
     # the fusion dispatcher is a host thread: not capturable - unless the static schedule replaces it after the first step
     graph_capable = os.environ.get("PTD_HVD_STATIC", "1") == "1" and os.environ.get("HOROVOD_AUTOTUNE", "0") != "1"
 

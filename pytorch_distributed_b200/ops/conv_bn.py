@@ -1,9 +1,14 @@
 """``conv1x1_bn_act``: 1x1 convolution -> BatchNorm (+ residual) (+ ReLU) with the BN statistics produced by the GEMM.
 
 The convolution runs as a hand-written wgmma GEMM (``csrc/gemm_bnstats.cu``: TMA -> smem -> ``wgmma.mma_async`` -> registers)
-whose epilogue reduces the per-channel sum / sum of squares of the stored bf16 output, so BatchNorm only needs its
+whose epilogue reduces the per-channel sum / sum of squares of the stored 16-bit output, so BatchNorm only needs its
 apply pass.  Backward: cuDNN dgrad / wgrad for the convolution, the fused BN backward kernels for the rest.
-Falls back to ``F.conv2d`` + :func:`bn_act` whenever the fast path does not apply (CPU, fp32/fp16, stride != 1, odd shapes).
+
+Training-mode steps take the GEMM when the activations and the weights are both bf16 or both fp16 (a model cast to
+bf16 / fp16, e.g. ``amp`` O2 / O3), and under ``torch.autocast("cuda")`` with a bf16 or fp16 autocast dtype (``amp`` O1,
+fp32 weights): there the weight is cast to the autocast dtype through autograd, as autocast's own ``F.conv2d`` would,
+so the fp32 parameter still receives an fp32 gradient.  Everything else - eval mode, CPU, fp32 activations, stride != 1,
+odd shapes, ``PTD_FUSED_CONV1X1=0`` - runs ``F.conv2d`` + :func:`bn_act`.
 """
 from __future__ import annotations
 
@@ -30,9 +35,27 @@ class _Conv1x1Stats(torch.autograd.Function):
         return dx, dw, None
 
 
+GEMM_DTYPES = (torch.bfloat16, torch.float16)
+
+
+def autocast_gemm_dtype():
+    """The dtype CUDA autocast runs convolutions in when it is enabled and one the GEMM takes (bf16 / fp16), else None."""
+    if torch.is_autocast_enabled("cuda"):
+        dt = torch.get_autocast_dtype("cuda")
+        if dt in GEMM_DTYPES:
+            return dt
+    return None
+
+
+def gemm_weight(w, autocast_dtype):
+    """The weight the GEMM multiplies by: ``w`` itself, or its autocast copy (a differentiable cast)."""
+    return w if autocast_dtype is None or w.dtype == autocast_dtype else w.to(autocast_dtype)
+
+
 def can_fuse_conv1x1(x, conv) -> bool:
     w = conv.weight
-    return (x.is_cuda and x.dtype == torch.bfloat16 and w.dtype == torch.bfloat16 and x.dim() == 4
+    wdt = autocast_gemm_dtype() or w.dtype
+    return (x.is_cuda and x.dtype in GEMM_DTYPES and wdt == x.dtype and w.is_floating_point() and x.dim() == 4
             and conv.kernel_size == (1, 1) and conv.stride == (1, 1) and conv.padding == (0, 0) and conv.groups == 1 and conv.bias is None
             and x.is_contiguous(memory_format=torch.channels_last) and x.size(1) % 64 == 0 and w.size(0) % 64 == 0
             and x.size(0) * x.size(2) * x.size(3) >= 128)
@@ -46,7 +69,7 @@ def conv1x1_bn_act(x, conv, bn, residual=None, enabled=True, split=False):
     nc = conv.weight.size(0)
     ws = workspace(x.device)
     work, gen = ws.take(4 * nc)
-    y = _Conv1x1Stats.apply(x, conv.weight, work[: 2 * nc])
+    y = _Conv1x1Stats.apply(x, gemm_weight(conv.weight, autocast_gemm_dtype()), work[: 2 * nc])
     if not _can_fuse(y, bn.weight, residual, bn.running_mean):
         return bn(y, residual, split) if split else bn(y, residual)   # (cannot happen for the shapes accepted above)
     need_grad = torch.is_grad_enabled() and (y.requires_grad or bn.weight.requires_grad)

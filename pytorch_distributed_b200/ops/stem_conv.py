@@ -3,13 +3,17 @@
 cuDNN runs this layer on legacy kernels (C_in = 3 fits no tensor-core tile).  Here
 (``csrc/stem_conv.cu``, ``csrc/gemm_bnstats.cu``):
 
-    A  = im2col(x)                    [M, 192] bf16, one 384-byte row per output pixel, k = r*24 + s*3 + c
+    A  = im2col(x)                    [M, 192] bf16 / fp16, one 384-byte row per output pixel, k = r*24 + s*3 + c
     y  = A @ Wp^T  (+ BN statistics)  persistent wgmma GEMM; the sums BatchNorm needs come out of its epilogue
     -> BN + ReLU + MaxPool            ``stem_forward_pre`` (the statistics pass of the fused stem tail is skipped)
     dW = unpack(dY^T @ A)             library GEMM over the saved A
 
-Opt-in (``PTD_STEM_GEMM=1`` / ``models.resnet.STEM_GEMM``) until it has been timed on hardware; the PyTorch functions
-below define the layout and are what the CPU tests check against ``F.conv2d``.
+On by default for training-mode forwards (``PTD_STEM_GEMM=0`` / ``models.resnet.STEM_GEMM = False`` restores cuDNN).  It
+runs when the image and the weight are both bf16 or both fp16 (a model cast to bf16 / fp16, e.g. ``amp`` O2 / O3), and
+under ``torch.autocast("cuda")`` with a bf16 or fp16 autocast dtype (``amp`` O1, fp32 weights and images): there the
+image and the weight are cast to the autocast dtype (the weight through autograd, so the fp32 parameter receives an fp32
+gradient), as autocast's own ``F.conv2d`` would.  Eval mode keeps cuDNN.  The PyTorch functions below define the layout
+and are what the CPU tests check against ``F.conv2d``.
 """
 from __future__ import annotations
 
@@ -17,6 +21,7 @@ import torch
 import torch.nn.functional as F
 
 from .bn_act import workspace
+from .conv_bn import GEMM_DTYPES, autocast_gemm_dtype, gemm_weight
 from .stem import _StemFn, bn_relu_maxpool, can_fuse_stem
 
 K_PAD = 192        # GEMM K: 7 filter rows x 24 (21 real elements each) = 168, padded to 3 x 64
@@ -54,7 +59,9 @@ def im2col_reference(x: torch.Tensor) -> torch.Tensor:
 
 def can_use_stem_gemm(x: torch.Tensor, conv) -> bool:
     w = conv.weight
-    return (x.is_cuda and x.dtype == torch.bfloat16 and w.dtype == torch.bfloat16 and x.dim() == 4 and x.size(1) == 3
+    ac = autocast_gemm_dtype()
+    xdt, wdt = (ac, ac) if ac is not None and x.is_floating_point() and w.is_floating_point() else (x.dtype, w.dtype)
+    return (x.is_cuda and xdt in GEMM_DTYPES and wdt == xdt and x.dim() == 4 and x.size(1) == 3
             and not x.requires_grad and conv.kernel_size == (7, 7) and conv.stride == (2, 2) and conv.padding == (3, 3)
             and conv.dilation == (1, 1) and conv.groups == 1 and conv.bias is None and w.size(0) % 64 == 0
             and x.is_contiguous(memory_format=torch.channels_last) and x.size(2) >= 7 and x.size(3) >= 7)
@@ -130,9 +137,12 @@ def stem_conv_bn_relu_maxpool(x, conv, bn, emulate: bool = False):
         y = _StemConvFn.apply(x, conv.weight, None, True)
         return bn_relu_maxpool(y, bn.weight, bn.bias, bn.running_mean, bn.running_var, training=True, momentum=momentum, eps=bn.eps,
                                fused=False, num_batches_tracked=nbt)
+    ac = autocast_gemm_dtype()
+    if ac is not None and x.dtype != ac:
+        x = x.to(ac)                                                   # keeps channels_last
     ws = workspace(x.device)
     work, gen = ws.take(4 * nc)
-    y = _StemConvFn.apply(x, conv.weight, work[: 2 * nc], False)      # always 4 inputs: backward returns 4 gradients
+    y = _StemConvFn.apply(x, gemm_weight(conv.weight, ac), work[: 2 * nc], False)   # always 4 inputs: backward returns 4 gradients
     if not can_fuse_stem(y, bn.weight, bn.running_mean):
         raise RuntimeError("stem GEMM output does not fit the fused stem tail")
     need_grad = torch.is_grad_enabled() and (y.requires_grad or bn.weight.requires_grad)

@@ -1,4 +1,7 @@
-"""Correctness + speed of the wgmma 1x1-conv GEMM with fused BN statistics against cuDNN conv + bn_stats."""
+"""Correctness + speed of the wgmma 1x1-conv GEMM with fused BN statistics against cuDNN conv + bn_stats.
+
+    PROBE_B=256 PROBE_DTYPE=bf16|fp16 python tools/gemm_probe.py       # on an H100; cuDNN runs in the same dtype
+"""
 import sys, os
 import torch
 import torch.nn.functional as F
@@ -7,6 +10,7 @@ from pytorch_distributed_b200 import _ext
 C = _ext.lib()
 torch.backends.cudnn.benchmark = True
 B = int(os.environ.get("PROBE_B", "256"))
+DT = {"bf16": torch.bfloat16, "fp16": torch.float16}[os.environ.get("PROBE_DTYPE", "bf16")]
 shapes = [(64, 64, 56), (64, 256, 56), (256, 64, 56), (256, 128, 56), (128, 512, 28), (512, 128, 28), (512, 256, 28), (256, 1024, 14),
           (1024, 256, 14), (1024, 512, 14), (512, 2048, 7), (2048, 512, 7)]
 if len(sys.argv) > 1 and sys.argv[1] == "small":
@@ -29,8 +33,8 @@ def t(fn, n=10):
 tot = [0.0, 0.0, 0.0]
 for cin, cout, hw in shapes:
     torch.manual_seed(0)
-    x = torch.randn(B, cin, hw, hw, device="cuda").bfloat16().contiguous(memory_format=torch.channels_last)
-    w = (torch.randn(cout, cin, 1, 1, device="cuda") * 0.1).bfloat16().contiguous(memory_format=torch.channels_last)
+    x = torch.randn(B, cin, hw, hw, device="cuda").to(DT).contiguous(memory_format=torch.channels_last)
+    w = (torch.randn(cout, cin, 1, 1, device="cuda") * 0.1).to(DT).contiguous(memory_format=torch.channels_last)
     gs = torch.zeros(2 * cout, device="cuda")
     y = C.conv1x1_bnstats(x, w, gs)
     torch.cuda.synchronize()
@@ -45,7 +49,7 @@ for cin, cout, hw in shapes:
         t_mine = t(lambda: C.conv1x1_bnstats(x, w, gs))
         t_conv = t(lambda: F.conv2d(x, w))
         work = torch.zeros(2 * cout, device="cuda")
-        wt, bt = torch.ones(cout, device="cuda", dtype=torch.bfloat16), torch.zeros(cout, device="cuda", dtype=torch.bfloat16)
+        wt, bt = torch.ones(cout, device="cuda", dtype=DT), torch.zeros(cout, device="cuda", dtype=DT)
         yc = F.conv2d(x, w)
         from pytorch_distributed_b200.ops.bn_act import bn_act, begin_step
         def both():
@@ -56,4 +60,5 @@ for cin, cout, hw in shapes:
         line += " | gemm+stats %.1f us, cudnn conv %.1f us, cudnn conv + bn_stats + bn_apply %.1f us" % (t_mine, t_conv, t_both)
     print(line, flush=True)
 if len(shapes) > 3:
+    print("%s, batch %d" % (str(DT).replace("torch.", ""), B))
     print("sum: gemm+stats %.1f us | cudnn conv %.1f us | conv+stats+apply %.1f us" % tuple(tot))

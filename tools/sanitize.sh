@@ -16,6 +16,10 @@ compute-sanitizer --tool memcheck --error-exitcode 9 python -m pytest tests/test
 echo "memcheck(gemm_bnstats, a CTA's second m-tile) exit $?"
 compute-sanitizer --tool racecheck --error-exitcode 9 python -m pytest tests/test_gpu_fp64.py -q -x -k "rpb3_odd_13x14_fp16_c32" -p no:cacheprovider
 echo "racecheck(stem backward, quad rows crossing images) exit $?"
+compute-sanitizer --tool memcheck --error-exitcode 9 python -m pytest tests/test_gpu_fp16_gemm.py -q -x -k "geometry_edges and one_cta_second_tile_n64" -p no:cacheprovider
+echo "memcheck(fp16 gemm_bnstats, a CTA's second m-tile) exit $?"
+compute-sanitizer --tool racecheck --error-exitcode 9 python -m pytest tests/test_gpu_fp16_gemm.py -q -x -k "stem_im2col and staged_224" -p no:cacheprovider
+echo "racecheck(fp16 staged stem_im2col) exit $?"
 compute-sanitizer --tool memcheck --error-exitcode 9 python -m pytest tests/test_gpu_data.py -q -x -k "equals_host_resample" -p no:cacheprovider
 echo "memcheck(resample) exit $?"
 compute-sanitizer --tool racecheck --error-exitcode 9 python -m pytest "tests/test_gpu_data.py::test_device_resample_equals_host_resample[True]" -q -x -p no:cacheprovider

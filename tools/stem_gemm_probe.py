@@ -1,6 +1,7 @@
 """Stem convolution: cuDNN (fprop / wgrad) vs im2col + wgmma GEMM (+BN statistics) + library wgrad, CUDA-event timings.
 
-    python tools/stem_gemm_probe.py [batch]        # on an H100; prints one markdown table
+    PROBE_DTYPE=bf16|fp16 python tools/stem_gemm_probe.py [batch]   # on an H100; prints one markdown table; cuDNN runs
+                                                                    # in the same dtype
 """
 import os
 import sys
@@ -33,8 +34,9 @@ def main():
     C = _ext.lib()
     torch.backends.cudnn.benchmark = True
     dev = torch.device("cuda", 0)
-    x = torch.randn(n, 3, 224, 224, device=dev).bfloat16().contiguous(memory_format=torch.channels_last)
-    w = torch.randn(64, 3, 7, 7, device=dev).bfloat16().contiguous(memory_format=torch.channels_last)
+    dt = {"bf16": torch.bfloat16, "fp16": torch.float16}[os.environ.get("PROBE_DTYPE", "bf16")]
+    x = torch.randn(n, 3, 224, 224, device=dev).to(dt).contiguous(memory_format=torch.channels_last)
+    w = (torch.randn(64, 3, 7, 7, device=dev) * 0.1).to(dt).contiguous(memory_format=torch.channels_last)
     y_ref = F.conv2d(x, w, stride=2, padding=3)
     dy = torch.randn_like(y_ref)
     stats = torch.zeros(128, device=dev)
@@ -51,7 +53,7 @@ def main():
     m = rows.size(0)
     gb_a = m * K_PAD * 2 / 1e9
     gb_y = m * 64 * 2 / 1e9
-    print("batch %d, M = %d, rel err y %.2e, dW %.2e" % (n, m, err, werr))
+    print("%s, batch %d, M = %d, rel err y %.2e, dW %.2e" % (str(dt).replace("torch.", ""), n, m, err, werr))
     print("| step | us | GB moved | GB/s |")
     print("|---|---:|---:|---:|")
     t = timed(lambda: F.conv2d(x, w, stride=2, padding=3))
@@ -65,7 +67,7 @@ def main():
     t = timed(lambda: torch.mm(dy2.t(), rows, out_dtype=torch.float32))
     print("| library wgrad GEMM (dY^T x A), fp32 out | %.0f | %.2f | %.0f |" % (t, gb_a + gb_y, (gb_a + gb_y) / t * 1e6))
     t = timed(lambda: dy2.t() @ rows)
-    print("| library wgrad GEMM (dY^T x A), bf16 out | %.0f | %.2f | %.0f |" % (t, gb_a + gb_y, (gb_a + gb_y) / t * 1e6))
+    print("| library wgrad GEMM (dY^T x A), 16-bit out | %.0f | %.2f | %.0f |" % (t, gb_a + gb_y, (gb_a + gb_y) / t * 1e6))
     t = timed(lambda: pack_stem_weight(w))
     print("| weight packing (ATen) | %.0f | | |" % t)
 
