@@ -499,13 +499,14 @@ __global__ void __launch_bounds__(1024) metrics_kernel(const __grid_constant__ C
   for (int r = warp; r < batch; r += nwarps) {
     const T* row = logits + (int64_t)r * row_stride;
     const int64_t t = target[r];
-    const float tv = (t >= 0 && t < classes) ? ldf(row + t) : INFINITY;
+    const bool valid = t >= 0 && t < classes;      // a target outside [0, classes) is never correct
+    const float tv = valid ? ldf(row + t) : INFINITY;
     int cnt = 0;
     for (int j = lane; j < classes; j += 32) cnt += (ldf(row + j) > tv) ? 1 : 0;
 #pragma unroll
     for (int o = 16; o; o >>= 1) cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
-    top1 += (cnt < 1);
-    top5 += (cnt < 5);
+    top1 += valid && cnt < 1;
+    top5 += valid && cnt < 5;
   }
   if (lane == 0) { atomicAdd(&s_top1, top1); atomicAdd(&s_top5, top5); }
   __syncthreads();

@@ -11,8 +11,11 @@
 //                     traffic with a bf16 arena: 2 R grad + 4 R/W master + 4 R/W momentum + 2 W model).
 //   fused_sgd_multi : classic chunked multi-tensor-apply over arbitrary tensor lists.
 //
-// Hyper-parameters live in a device tensor `hyper` = {lr, momentum, weight_decay, dampening, grad_multiplier}
-// so a captured CUDA graph keeps working when the LR schedule or the loss scale changes.
+// Hyper-parameters live in a device tensor `hyper` = {lr, momentum, weight_decay, dampening, grad_multiplier,
+// momentum_pending} so a captured CUDA graph keeps working when the LR schedule or the loss scale changes.
+// momentum_pending (slot 5) is read only under dynamic loss scaling (a found_inf flag is given): while it is non-zero the
+// step initialises the momentum buffer (m = g), as on the first step.  amp_update_scale clears it after the first step
+// that was applied, so a skipped (overflowed) first step does not turn the next one into m = (1 - dampening) g.
 #include <ATen/cuda/CUDAContext.h>
 #include <c10/cuda/CUDAGuard.h>
 #include <torch/extension.h>
@@ -42,6 +45,7 @@ __global__ void __launch_bounds__(256) fused_sgd_flat_kernel(const G* __restrict
                                                              bool nesterov, bool first) {
   if (found_inf && *found_inf) return;  // dynamic loss scaling: skip the step on overflow
   const SgdHyper h = load_hyper(hyper);
+  first = first || (found_inf && hyper[5] != 0.f);
   const int64_t nvec = n >> 3;
   for (int64_t v = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; v < nvec; v += (int64_t)gridDim.x * blockDim.x) {
     float g[8], p[8], m[8];
@@ -64,6 +68,7 @@ void fused_sgd_flat(at::Tensor grad, at::Tensor master, at::Tensor momentum, c10
   TORCH_CHECK(grad.numel() >= n && momentum.numel() == n, "flat buffer size mismatch");
   TORCH_CHECK(master.scalar_type() == at::kFloat && momentum.scalar_type() == at::kFloat && hyper.scalar_type() == at::kFloat);
   TORCH_CHECK(master.is_contiguous() && momentum.is_contiguous() && grad.is_contiguous());
+  TORCH_CHECK(!found_inf.has_value() || hyper.numel() >= 6, "hyper needs slot 5 (momentum_pending) when found_inf is given");
   c10::cuda::CUDAGuard guard(master.device());
   const int* fi = found_inf.has_value() ? reinterpret_cast<const int*>(found_inf->data_ptr()) : nullptr;
   const int sms = at::cuda::getCurrentDeviceProperties()->multiProcessorCount;
@@ -134,6 +139,7 @@ __global__ void __launch_bounds__(256) fused_sgd_multi_kernel(const __grid_const
                                                               const int* __restrict__ found_inf, bool nesterov, bool first) {
   if (found_inf && *found_inf) return;
   const SgdHyper h = load_hyper(hyper);
+  first = first || (found_inf && hyper[5] != 0.f);
   const int t = a.block_tensor[blockIdx.x];
   const int64_t begin = (int64_t)a.block_chunk[blockIdx.x] * kMtaChunk;
   const int64_t end = min(begin + (int64_t)kMtaChunk, a.numel[t]);
@@ -231,6 +237,7 @@ void fused_sgd_multi(std::vector<at::Tensor> grads, std::vector<at::Tensor> para
   TORCH_CHECK(model_copies.empty() || model_copies.size() == params.size());
   for (auto& p : params) TORCH_CHECK(p.scalar_type() == at::kFloat, "params (masters) must be fp32");
   for (auto& m : momenta) TORCH_CHECK(m.scalar_type() == at::kFloat, "momentum must be fp32");
+  TORCH_CHECK(!found_inf.has_value() || hyper.numel() >= 6, "hyper needs slot 5 (momentum_pending) when found_inf is given");
   c10::cuda::CUDAGuard guard(params[0].device());
   cudaStream_t st = at::cuda::getCurrentCUDAStream();
   const int* fi = found_inf.has_value() ? reinterpret_cast<const int*>(found_inf->data_ptr()) : nullptr;
@@ -267,10 +274,12 @@ void multi_tensor_axpby(std::vector<at::Tensor> x, std::vector<at::Tensor> y, st
 }
 
 // Dynamic loss-scale state machine on the device (apex semantics: x2 after `interval` clean steps, /2 and skip on
-// overflow).  Also refreshes hyper[4] = grad multiplier = 1/scale and clears found_inf for the next step.
+// overflow).  Also refreshes hyper[4] = grad multiplier = 1/scale, clears hyper[5] (momentum_pending) after an applied
+// step and clears found_inf for the next step.
 __global__ void amp_update_scale_kernel(float* scale, int* tracker, int* found_inf, float growth, float backoff, int interval, float* hyper,
-                                        float extra_mul) {
-  if (*found_inf) {
+                                        bool has_pending, float extra_mul) {
+  const bool bad = *found_inf != 0;
+  if (bad) {
     *scale = fmaxf(*scale * backoff, 1.0f);
     *tracker = 0;
   } else {
@@ -284,6 +293,7 @@ __global__ void amp_update_scale_kernel(float* scale, int* tracker, int* found_i
   }
   *found_inf = 0;
   if (hyper) hyper[4] = extra_mul / *scale;
+  if (has_pending && !bad) hyper[5] = 0.f;
 }
 
 void amp_update_scale(at::Tensor scale, at::Tensor growth_tracker, at::Tensor found_inf, double growth, double backoff, int64_t interval,
@@ -291,9 +301,10 @@ void amp_update_scale(at::Tensor scale, at::Tensor growth_tracker, at::Tensor fo
   TORCH_CHECK(scale.scalar_type() == at::kFloat && growth_tracker.scalar_type() == at::kInt && found_inf.scalar_type() == at::kInt);
   c10::cuda::CUDAGuard guard(scale.device());
   float* hp = hyper.defined() && hyper.numel() >= 5 ? hyper.data_ptr<float>() : nullptr;
+  const bool has_pending = hp && hyper.numel() >= 6;
   amp_update_scale_kernel<<<1, 1, 0, at::cuda::getCurrentCUDAStream()>>>(scale.data_ptr<float>(), growth_tracker.data_ptr<int>(),
                                                                          found_inf.data_ptr<int>(), (float)growth, (float)backoff,
-                                                                         (int)interval, hp, 1.0f);
+                                                                         (int)interval, hp, has_pending, 1.0f);
   C10_CUDA_KERNEL_LAUNCH_CHECK();
 }
 

@@ -232,7 +232,12 @@ class TrainStep:
         self.metrics.join()
         eng = getattr(self.st, "engine", None)
         if _POISON and eng is not None and getattr(eng, "_flat", None) is not None and getattr(eng, "fused", False):
-            eng.grad_arena().fill_(float("nan"))   # PTD_DEBUG_POISON=1: a stale read of the wire arena shows up as NaN
+            # PTD_DEBUG_POISON=1: a stale read of the wire arena shows up as NaN.  Only the parameters' own ranges are
+            # poisoned: the alignment padding is never packed, and NaN left there would trip the all-reduce's non-finite
+            # test (dynamic loss scaling) on every step
+            arena = eng.grad_arena()
+            for off, p in zip(eng.param_elem_off, eng.params):
+                arena[off:off + p.numel()].fill_(float("nan"))
 
     def _capture(self, images, target):
         self.static_x, self.static_y = images.clone(), target.clone()

@@ -113,7 +113,10 @@ class FusedSGD(Optimizer):
         vals = (float(group["lr"]), float(group["momentum"]), float(group["weight_decay"]), float(group["dampening"]))
         ent = self._hyper.get(gi)
         if ent is None:
-            t = torch.tensor(list(vals) + [gmul, 0, 0, 0], dtype=torch.float32, device=device)
+            # slot 5 (momentum_pending): under dynamic loss scaling the momentum is initialised by the first step that is
+            # actually applied; the loss scaler clears the slot after it (csrc/optim.cu)
+            pending = 1.0 if self._steps == 0 else 0.0
+            t = torch.tensor(list(vals) + [gmul, pending, 0, 0], dtype=torch.float32, device=device)
             self._hyper[gi] = [t, vals]
             return t
         if ent[1] != vals:
@@ -250,3 +253,5 @@ class FusedSGD(Optimizer):
             loaded = any("momentum_buffer" in st for st in self.state.values())
         if loaded:
             self._steps = max(self._steps, 1)      # do not re-initialise the momentum on the next step
+            for ent in self._hyper.values():
+                ent[0][5].fill_(0.0)

@@ -31,7 +31,8 @@ class LossScaler:
         self.tracker = torch.zeros(1, dtype=torch.int32, device=self.device)
         self.found_inf = torch.zeros(1, dtype=torch.int32, device=self.device)
         self.growth_factor, self.backoff_factor, self.growth_interval = growth_factor, backoff_factor, growth_interval
-        self._hyper = None
+        self._hyper = None            # hyper tensor attached last (the one amp_update_scale refreshes)
+        self._hypers = []             # every hyper tensor ever attached (one per FusedSGD param group)
         self.skipped_steps_host = 0   # only maintained on the host-synchronising (stock optimizer) path
 
     # ---- device-side protocol used by FusedSGD
@@ -44,16 +45,26 @@ class LossScaler:
         if self._hyper is not hyper:
             self._hyper = hyper
             hyper[4:5].copy_(1.0 / self.scale)
+        if not any(h is hyper for h in self._hypers):
+            self._hypers.append(hyper)
 
     def update(self) -> None:
         """Post-step: run the scale state machine, refresh 1/scale for the optimizer, clear the overflow flag."""
         if self.device.type == "cuda":
             from .. import _ext
             hyper = self._hyper if self._hyper is not None else torch.empty(0, device=self.device)
+            # every param group has its own hyper tensor; amp_update_scale refreshes the last attached one, the others get
+            # the same treatment here: momentum_pending (slot 5) stays set only if this step was skipped, and 1/scale (slot 4)
+            others = [h for h in self._hypers if h is not hyper or not self.dynamic]
+            for h in others:
+                if h.numel() >= 6:
+                    h[5:6].mul_(self.found_inf)
             if self.dynamic:
                 _ext.note_launch()
                 _ext.lib().amp_update_scale(self.scale, self.tracker, self.found_inf, self.growth_factor, self.backoff_factor,
                                             self.growth_interval, hyper)
+                for h in others:
+                    h[4:5].copy_(hyper[4:5])
             else:
                 self.found_inf.zero_()
         else:
@@ -68,8 +79,8 @@ class LossScaler:
                         self.scale.mul_(self.growth_factor)
                         self.tracker.zero_()
             self.found_inf.zero_()
-            if self._hyper is not None:
-                self._hyper[4:5].copy_(1.0 / self.scale)
+            for h in self._hypers:
+                h[4:5].copy_(1.0 / self.scale)
 
     # ---- host-synchronising helpers (CPU path and stock torch optimizers)
     def host_found_inf(self) -> bool:

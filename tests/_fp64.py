@@ -309,3 +309,130 @@ def stem_dz_ref(dp, code, H, W):
         kh, kw = divmod(k, 3)
         dzp[:, :, kh:kh + 2 * OH:2, kw:kw + 2 * OW:2] += torch.where(code == k, d, torch.zeros_like(d))
     return dzp[:, :, 1:H + 1, 1:W + 1]
+
+
+# ---------------------------------------------------------------------------------------------------------- optimizer
+# csrc/optim.cu: chunked multi-tensor apply (mta_for_each) and the flat SGD launch
+MTA_TENSORS, MTA_BLOCKS, MTA_CHUNK = 30, 320, 8192
+
+
+def sgd_step_fp64(p, m, g, hyper, nesterov: bool, first: bool) -> dict:
+    """One step of ``sgd_update`` (csrc/optim.cu) in float64 from the fp32 state the kernel started with: returns the new
+    master ``p``, momentum ``m``, and a bound on the kernel's error in each.
+
+    ``hyper`` = (lr, momentum, weight_decay, dampening, gmul) as the kernel read them (fp32 values).  The kernel computes
+        a = g*gmul + wd*p;  m' = first ? a : mom*m + (1 - d)*a;  b = nesterov ? a + mom*m' : m';  p' = p - lr*b
+    (momentum 0: b = a, m unchanged) with fp32 roundings of every product, sum and of (1 - d).  Each rounding adds at
+    most u |value rounded| (u = 2^-24); the errors carried into a later operation are scaled by its coefficient:
+        e_a  = u (|g gmul| + |wd p| + |a|)
+        e_m' = e_a                                              (first)
+             = u |mom m| + |1-d| e_a + 2 u |(1-d) a| + u |m'|   (otherwise)
+        e_b  = e_a + |mom| e_m' + u |mom m'| + u |b|            (nesterov),  e_m'  (plain),  e_a  (momentum 0)
+        e_p' = |lr| e_b + u |lr b| + u |p'|
+    An FMA contraction by nvcc removes roundings, so it only tightens this.  First-order terms only: the factor 1.01
+    covers the products of u, and 8 * 2^-126 covers results flushed to zero (the extension is built with --use_fast_math,
+    so subnormal fp32 results are flushed).  Compare one step at a time from the
+    kernel's own previous state, so that errors do not compound."""
+    lr, mom, wd, d, gmul = (float(x) for x in hyper[:5])
+    p, m, g = p.double(), m.double(), g.double()
+    tiny = 8 * 2.0 ** -126
+    a = g * gmul + wd * p
+    e_a = U32 * ((g * gmul).abs() + (wd * p).abs() + a.abs())
+    if mom != 0.0:
+        if first:
+            m1, e_m = a, e_a
+        else:
+            m1 = mom * m + (1.0 - d) * a
+            e_m = U32 * (mom * m).abs() + abs(1.0 - d) * e_a + 2 * U32 * ((1.0 - d) * a).abs() + U32 * m1.abs()
+        if nesterov:
+            b = a + mom * m1
+            e_b = e_a + abs(mom) * e_m + U32 * (mom * m1).abs() + U32 * b.abs()
+        else:
+            b, e_b = m1, e_m
+    else:
+        m1, e_m = m, torch.zeros_like(m)
+        b, e_b = a, e_a
+    p1 = p - lr * b
+    e_p = abs(lr) * e_b + U32 * (lr * b).abs() + U32 * p1.abs()
+    return dict(p=p1, m=m1, p_bound=1.01 * e_p + tiny, m_bound=1.01 * e_m + tiny)
+
+
+def check_sgd(name: str, p, m, ref: dict) -> float:
+    """Master and momentum against sgd_step_fp64; returns the largest error / bound ratio."""
+    assert_within(name + " master", p, ref["p"], ref["p_bound"])
+    assert_within(name + " momentum", m, ref["m"], ref["m_bound"])
+    rp = ((p.double() - ref["p"]).abs() / ref["p_bound"]).max().item()
+    rm = ((m.double() - ref["m"]).abs() / ref["m_bound"]).max().item()
+    return max(rp, rm)
+
+
+def mta_geometry(numels) -> list:
+    """mta_for_each (csrc/optim.cu): the launches of a multi-tensor kernel over tensors of the given sizes.
+
+    Each launch is a dict: ``tensors`` (indices registered, in order; a tensor split across launches is registered again
+    in the next one), ``ranges`` (tensor -> [first chunk, last chunk + 1) of MTA_CHUNK elements handled in this launch),
+    ``blocks`` (CTAs) and ``reason`` - why the launch was flushed: "tensors" (MTA_TENSORS registered), "blocks"
+    (MTA_BLOCKS CTAs) or "end" (the list ran out).  Zero-size tensors are skipped."""
+    launches = []
+    cur = dict(tensors=[], ranges={}, blocks=0)
+
+    def flush(reason):
+        nonlocal cur
+        if cur["blocks"] > 0:
+            cur["reason"] = reason
+            launches.append(cur)
+        cur = dict(tensors=[], ranges={}, blocks=0)
+
+    for i, n in enumerate(int(x) for x in numels):
+        if n == 0:
+            continue
+        chunks = cdiv(n, MTA_CHUNK)
+        c = 0
+        while c < chunks:
+            if len(cur["tensors"]) == MTA_TENSORS or cur["blocks"] == MTA_BLOCKS:
+                flush("tensors" if len(cur["tensors"]) == MTA_TENSORS else "blocks")
+            take = min(chunks - c, MTA_BLOCKS - cur["blocks"])
+            cur["tensors"].append(i)
+            cur["ranges"][i] = (c, c + take)
+            cur["blocks"] += take
+            c += take
+    flush("end")
+    return launches
+
+
+def sgd_flat_geometry(n: int, sms: int) -> dict:
+    """fused_sgd_flat: 8 elements per thread-iteration, 256 threads, grid = min(ceil(n/8 / 256), 8 * SMs); a thread takes
+    up to ``iters`` grid-stride iterations."""
+    nvec = n // 8
+    grid = min(cdiv(nvec, 256), sms * 8)
+    return dict(grid=grid, iters=cdiv(nvec, grid * 256), nvec=nvec)
+
+
+def wire_round(src: torch.Tensor, scale: float, wire) -> torch.Tensor:
+    """What pack writes for ``src``: fp32(src) * fp32(scale), rounded to nearest even into the wire dtype (torch's casts
+    round like __float2bfloat16_rn / __float2half_rn, including fp16 overflow to +-inf and fp16 subnormals)."""
+    return (src.float() * float(scale)).to(wire)
+
+
+def assert_bits_equal(name: str, got: torch.Tensor, ref: torch.Tensor) -> None:
+    """Bitwise equality of two tensors of the same floating dtype (any NaN equals any NaN)."""
+    assert got.dtype == ref.dtype, "%s: dtype %s != %s" % (name, got.dtype, ref.dtype)
+    g, r = got.reshape(-1), ref.reshape(-1)
+    ib = {2: torch.int16, 4: torch.int32, 8: torch.int64}[g.element_size()]
+    diff = (g.view(ib) != r.view(ib)) & ~(torch.isnan(g) & torch.isnan(r))
+    n = int(diff.sum())
+    if n:
+        i = int(diff.to(torch.int8).argmax())
+        raise AssertionError("%s: %d of %d elements differ bitwise; first at flat index %d: got %r, expected %r"
+                             % (name, n, g.numel(), i, g[i].item(), r[i].item()))
+
+
+def topk_correct_ref(logits: torch.Tensor, target: torch.Tensor, ks=(1, 5)) -> list:
+    """utils/meters.accuracy's rule as exact integers: sample i is top-k correct iff its target lies in [0, classes) and
+    fewer than k logits are strictly greater than the target logit (16-bit and fp32 logits are exact in float64)."""
+    x = logits.double()
+    C = x.size(1)
+    valid = (target >= 0) & (target < C)
+    tv = x.gather(1, target.clamp(0, max(C - 1, 0)).view(-1, 1))
+    rank = (x > tv).sum(1)
+    return [int((valid & (rank < k)).sum()) for k in ks]
