@@ -145,13 +145,15 @@ __device__ __forceinline__ bool unpack_block(const PtrPack& pk, const PlanArgs& 
 }
 
 // Sum the 16-byte unit at byte offset `off` over all ranks with plain peer loads (fp32 accumulation).
+// The adds run in rank order 0..world-1 on EVERY rank, so the result is a fixed function of the inputs: the one-shot
+// kernel's ranks (each reduces the whole range itself) hold the same bits and take the same non-finite decision, and
+// the two-shot / reduce-to-caller results do not depend on which rank owns a slice or calls.
 template <typename W>
 __device__ __forceinline__ void p2p_reduce_unit(const CommCtx& c, int64_t off, float (&acc)[sizeof(W) == 4 ? 4 : 8]) {
   constexpr int N = sizeof(W) == 4 ? 4 : 8;
 #pragma unroll
   for (int k = 0; k < N; ++k) acc[k] = 0.f;
-  for (int i = 0; i < c.world; ++i) {
-    const int p = (c.rank + i) % c.world;  // stagger peers so the ranks do not all hit the same GPU first
+  for (int p = 0; p < c.world; ++p) {
     V4 v = ld_sys(c.base[p] + off);
     if constexpr (sizeof(W) == 4) {
       acc[0] += __uint_as_float(v.x); acc[1] += __uint_as_float(v.y); acc[2] += __uint_as_float(v.z); acc[3] += __uint_as_float(v.w);
@@ -331,7 +333,9 @@ __global__ void __launch_bounds__(kThreads) oneshot_allreduce_kernel(const __gri
     }
   }
   if (a.found_inf && __syncthreads_or(bad) && threadIdx.x == 0) {
-    // every rank reduced the same values, so every rank takes the same decision: a local store is enough
+    // every rank reduced the same values in the same order (rank order on P2P; on NVLS the switch's sum, which
+    // tests/mp_gpu_checks.py requires to be identical across ranks), so every rank takes the same decision: a local store
+    // is enough
     *reinterpret_cast<volatile uint32_t*>(a.found_inf) = 1u;
   }
   __syncthreads();

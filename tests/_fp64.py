@@ -427,6 +427,89 @@ def assert_bits_equal(name: str, got: torch.Tensor, ref: torch.Tensor) -> None:
                              % (name, n, g.numel(), i, g[i].item(), r[i].item()))
 
 
+# ---------------------------------------------------------------------------------------------------------- collectives
+# csrc/collectives.cu: 512 threads per CTA, 16-byte units; one-shot and reduce-to-caller keep 8 units in flight per thread,
+# push_range 4; the two-shot P2P reduce is a single grid-stride loop.
+COLL_THREADS = 512
+ONESHOT_U, REDUCE_U, PUSH_U = 8, 8, 4
+
+
+def allreduce_ref(per_rank_wire, wire=None, scale: float = 1.0, prepacked: bool = False) -> torch.Tensor:
+    """The P2P reduce contract of every rank: the fp32 sum, in rank order 0..W-1 starting from +0.0, of the values each
+    rank put on the wire; with ``prepacked`` (the scale was not applied by a pack pass) the fp32 product with fp32(scale);
+    then one rounding to the wire dtype.  Inputs are the per-rank wire tensors (same shape and dtype)."""
+    wire = per_rank_wire[0].dtype if wire is None else wire
+    acc = torch.zeros(per_rank_wire[0].shape, dtype=torch.float32, device=per_rank_wire[0].device)
+    for v in per_rank_wire:
+        acc = acc + v.float()
+    if prepacked:
+        acc = acc * torch.tensor(scale, dtype=torch.float32, device=acc.device)
+    return acc.to(wire)
+
+
+def staggered_ref(per_rank_wire, rank: int) -> torch.Tensor:
+    """Host model of a reduction that starts at the caller's own rank, p = (rank + i) mod W: the order the P2P reduce
+    used before it summed in rank order.  Kept to show that the bitwise checks can tell the two orders apart."""
+    W = len(per_rank_wire)
+    acc = torch.zeros(per_rank_wire[0].shape, dtype=torch.float32, device=per_rank_wire[0].device)
+    for i in range(W):
+        acc = acc + per_rank_wire[(rank + i) % W].float()
+    return acc.to(per_rank_wire[0].dtype)
+
+
+def slice_owner(layout, pos):
+    """Rank that reduces arena element ``pos`` (int or int64 tensor) in the two-shot kernel: CTA b = pos // block_elems
+    owns [b * block_elems, (b + 1) * block_elems) and rank r owns the r-th of its ``world`` equal slices."""
+    slice_elems = layout.block_elems // layout.world
+    return (pos % layout.block_elems) // slice_elems
+
+
+def loop_units(units: int, U: int, threads: int = COLL_THREADS) -> dict:
+    """How a CTA's ``units`` 16-byte units split between an unrolled main loop (``for (u = tid; u + (U-1)*T < units;
+    u += U*T)``) and the single-unit tail loop that follows it."""
+    main = tail = 0
+    for t in range(min(threads, units)):
+        n = 0 if t + (U - 1) * threads >= units else (units - (U - 1) * threads - 1 - t) // (U * threads) + 1
+        main += n * U
+        tail += len(range(t + n * U * threads, units, threads))
+    assert main + tail == units
+    return dict(units=units, main_units=main, tail_units=tail)
+
+
+def oneshot_units(layout, wire_bytes: int) -> dict:
+    """oneshot_allreduce_kernel (and reduce_to_caller_kernel, same U): every rank reduces the whole CTA range."""
+    return loop_units(layout.block_elems * wire_bytes // 16, ONESHOT_U)
+
+
+def push_units(layout, wire_bytes: int) -> dict:
+    """push_range of fused_broadcast_kernel / push_kernel."""
+    return loop_units(layout.block_elems * wire_bytes // 16, PUSH_U)
+
+
+def twoshot_units(layout, wire_bytes: int) -> dict:
+    """fused_allreduce_kernel (P2P): each rank reduces its slice of every CTA range, one unit per loop iteration."""
+    units = layout.block_elems // layout.world * wire_bytes // 16
+    return dict(units=units, main_units=units, tail_units=0, iters=cdiv(units, COLL_THREADS))
+
+
+def ll_allreduce_ref(per_rank_in, scale: float) -> torch.Tensor:
+    """ll_allreduce_kernel: slot s is the fp32 sum over sources in rank order (from +0.0) times fp32(scale)."""
+    acc = torch.zeros_like(per_rank_in[0], dtype=torch.float32)
+    for v in per_rank_in:
+        acc = acc + v.float()
+    return acc * torch.tensor(scale, dtype=torch.float32, device=acc.device)
+
+
+def metrics_mean_bound(vals: torch.Tensor, world: int, got: torch.Tensor) -> tuple:
+    """metrics_kernel's cross-rank mean of ``vals`` [world, 3] (fp32 values the ranks sent): returns the fp64 mean and
+    a bound.  Lane l < 3W of warp 0 takes term l, and l + 32 when 3W > 32, then a 5-level xor-shuffle tree: depth
+    cdiv(3W, 32) + 5 additions.  The division by ``world`` is a --use_fast_math '/', within 2 ulp of the result."""
+    v = vals.double()
+    depth = cdiv(3 * world, 32) + 5
+    ref = v.sum(0) / world
+    return ref, 1.01 * depth * U32 * v.abs().sum(0) / world + 2 * ulp(got, torch.float32)
+
+
 def topk_correct_ref(logits: torch.Tensor, target: torch.Tensor, ks=(1, 5)) -> list:
     """utils/meters.accuracy's rule as exact integers: sample i is top-k correct iff its target lies in [0, classes) and
     fewer than k logits are strictly greater than the target logit (16-bit and fp32 logits are exact in float64)."""

@@ -53,6 +53,13 @@ def main():
                     t_eff = max(tol, {torch.bfloat16: 1e-2, torch.float16: 2e-3}.get(w.dtype, 0.0))   # destination rounding
                     lim = t_eff * max(1.0, r.abs().max().item())
                     assert err <= lim, "allreduce wire=%s kind=%d nvls=%s: err %g > %g" % (wire, kind, nvls, err, lim)
+                # every rank must hold the same bits: P2P sums in rank order on every rank, and multimem.ld_reduce must
+                # return one sum to every requester
+                flat = torch.cat([w.reshape(-1).float() for w in work])
+                every = [torch.empty_like(flat) for _ in range(world)]
+                dist.all_gather(every, flat)
+                for q in range(1, world):
+                    assert torch.equal(every[q], every[0]), "allreduce wire=%s kind=%d nvls=%s: rank %d differs from rank 0" % (wire, kind, nvls, q)
 
     # ---- generic API: all_reduce_ (small => one-shot, large => two-shot), broadcast_
     a = torch.full((10,), float(rank + 1), device=dev)
