@@ -14,6 +14,8 @@ import torch.nn as nn
 from ...parallel import amp as _amp
 from ...parallel.comm import make_communicator
 from ...parallel.ddp import GradientEngine, _float_buffers, sync_module_states
+from ...utils.dist_ops import register_for_sync_batchnorm
+from ...models.resnet import SyncBNAct, convert_sync_batchnorm
 
 _WIRE = {torch.float16: "fp16", torch.bfloat16: "bf16", torch.float32: "fp32"}
 
@@ -53,6 +55,7 @@ class DistributedDataParallel(nn.Module):
         if isinstance(comm, str):
             comm = make_communicator(comm, group=process_group, device=device)
         self.comm = comm
+        register_for_sync_batchnorm(module, comm)
         scaler = _amp.current_scaler()
         if wire_dtype is None:
             if allreduce_always_fp32 or device.type != "cuda":
@@ -123,3 +126,25 @@ def unflatten(flat, tensors):
         out.append(flat.narrow(0, off, n).view_as(t))
         off += n
     return out
+
+
+class SyncBatchNorm(SyncBNAct):
+    """apex.parallel.SyncBatchNorm: apex's signature over the synchronised fused BatchNorm.  ``fuse_relu`` applies the
+    ReLU inside the layer (``forward(x, z)`` adds ``z`` first, as apex's); ``channel_last`` is accepted for parity: the fused
+    kernels take channels_last activations whatever it says, other layouts run torch's synchronised BatchNorm."""
+
+    def __init__(self, num_features, eps=1e-5, momentum=0.1, affine=True, track_running_stats=True, process_group=None,
+                 channel_last=False, fuse_relu=False):
+        super().__init__(num_features, eps=eps, momentum=momentum, affine=affine, track_running_stats=track_running_stats,
+                         process_group=process_group, relu=bool(fuse_relu))
+        self.channel_last = channel_last
+
+    def forward(self, input, z=None):  # type: ignore[override]
+        return super().forward(input, z)
+
+
+def convert_syncbn_model(module: nn.Module, process_group=None, channel_last: bool = False) -> nn.Module:
+    """apex.parallel.convert_syncbn_model: every BatchNorm layer of ``module`` becomes a synchronised one (``SyncBatchNorm``,
+    sharing its Parameters and buffers).  ``channel_last`` is accepted for signature parity: the fused kernels take
+    channels_last activations whatever it says, other layouts run torch's synchronised BatchNorm."""
+    return convert_sync_batchnorm(module, process_group)

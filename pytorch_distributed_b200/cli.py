@@ -88,6 +88,9 @@ def build_parser(entry: str = "distributed") -> argparse.ArgumentParser:
     x.add_argument("--optimizer", default="fused", choices=["fused", "torch"],
                    help="fused = hand-written multi-tensor SGD kernel; torch = torch.optim.SGD")
     x.add_argument("--cuda-graph", action="store_true", help="capture the train step in a CUDA graph")
+    x.add_argument("--sync-bn", action="store_true",
+                   help="synchronise BatchNorm statistics across the data-parallel ranks (torch.nn.SyncBatchNorm semantics; "
+                        "fused into the BN kernels with --comm fused)")
     x.add_argument("--overlap-optimizer", dest="overlap_optimizer", action="store_true", default=True,
                    help="fused optimizer: update each gradient bucket right behind its all-reduce, inside backward (default)")
     x.add_argument("--no-overlap-optimizer", dest="overlap_optimizer", action="store_false")

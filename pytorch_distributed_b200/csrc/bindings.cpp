@@ -37,7 +37,15 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.attr("MAX_PTRS") = kMaxPtrs;
   m.attr("SIGNAL_PAD_BYTES") = (int64_t)sizeof(SignalPad);
   m.attr("SEG_BYTES") = (int64_t)sizeof(Seg);
+  m.attr("SYNC_BN_MAX_C") = kSyncBnMaxC;
+  m.attr("SYNC_BN_AREA_BYTES") = kSyncBnAreaBytes;
   m.def("multicast_supported", &multicast_supported);
+
+  // handle of a synchronised BatchNorm layer group: the peers' context, the exchange area offset, the call counters
+  py::class_<SyncBN>(m, "SyncBN")
+      .def_property_readonly("rank", [](const SyncBN& s) { return s.ctx.rank; })
+      .def_property_readonly("world", [](const SyncBN& s) { return s.ctx.world; })
+      .def_property_readonly("xoff", [](const SyncBN& s) { return s.xoff; });
 
   py::class_<SymmArena, std::shared_ptr<SymmArena>>(m, "SymmArena")
       .def(py::init<int, int, int, int64_t>(), py::arg("device"), py::arg("rank"), py::arg("world"), py::arg("bytes"))
@@ -87,7 +95,14 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
            })
       .def("launch_ll_allreduce", [](std::shared_ptr<SymmArena> a, int channel, const at::Tensor& in, at::Tensor out, double scale) {
         launch_ll_allreduce(a->ctx(channel), in, out, scale, a->ll_seq_ptr());
-      });
+      })
+      .def("sync_bn",
+           [](std::shared_ptr<SymmArena> a, int channel, int64_t xoff, int64_t calls_ptr, int as_rank) {
+             TORCH_CHECK(xoff >= 0 && xoff % 16 == 0 && xoff + kSyncBnAreaBytes <= a->bytes(), "sync BN exchange area outside the arena");
+             TORCH_CHECK(calls_ptr != 0, "sync BN call counters missing");
+             return SyncBN{a->ctx(channel, as_rank), xoff, reinterpret_cast<uint32_t*>(calls_ptr)};
+           },
+           py::arg("channel"), py::arg("xoff"), py::arg("calls_ptr"), py::arg("as_rank") = 0);
 
   m.def("pack_pointers", &pack_pointers);
   m.def("fused_sgd_flat", &fused_sgd_flat, py::arg("grad"), py::arg("master"), py::arg("momentum"), py::arg("model_copy"), py::arg("hyper"),
@@ -96,14 +111,23 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("multi_tensor_scale", &multi_tensor_scale);
   m.def("multi_tensor_axpby", &multi_tensor_axpby);
   m.def("amp_update_scale", &amp_update_scale);
-  m.def("bn_act_forward", &bn_act_forward);
-  m.def("bn_act_backward", &bn_act_backward);
-  m.def("bn_act_backward2", &bn_act_backward2);
-  m.def("stem_forward", &stem_forward);
-  m.def("stem_forward_pre", &stem_forward_pre);
-  m.def("stem_backward", &stem_backward);
+  // BatchNorm entry points: `sync` (a SyncBN, default None = this rank alone) selects the synchronised variant
+  const auto sync_arg = py::arg("sync") = static_cast<const SyncBN*>(nullptr);
+  m.def("bn_act_forward", &bn_act_forward, py::arg("x"), py::arg("residual"), py::arg("weight"), py::arg("bias"), py::arg("running_mean"),
+        py::arg("running_var"), py::arg("num_batches_tracked"), py::arg("training"), py::arg("momentum"), py::arg("eps"), py::arg("relu"),
+        py::arg("need_mask"), py::arg("work"), py::arg("stats_ready"), sync_arg);
+  m.def("bn_act_backward", &bn_act_backward, py::arg("dy"), py::arg("x"), py::arg("mask"), py::arg("weight"), py::arg("saved"), py::arg("relu"),
+        py::arg("has_residual"), py::arg("work"), sync_arg);
+  m.def("bn_act_backward2", &bn_act_backward2, py::arg("dy_a"), py::arg("dy_b"), py::arg("x"), py::arg("mask"), py::arg("weight"),
+        py::arg("saved"), py::arg("relu"), py::arg("work"), sync_arg);
+  m.def("stem_forward", &stem_forward, py::arg("x"), py::arg("weight"), py::arg("bias"), py::arg("running_mean"), py::arg("running_var"),
+        py::arg("num_batches_tracked"), py::arg("training"), py::arg("momentum"), py::arg("eps"), py::arg("need_code"), py::arg("work"), sync_arg);
+  m.def("stem_forward_pre", &stem_forward_pre, py::arg("x"), py::arg("weight"), py::arg("bias"), py::arg("running_mean"), py::arg("running_var"),
+        py::arg("num_batches_tracked"), py::arg("training"), py::arg("momentum"), py::arg("eps"), py::arg("need_code"), py::arg("work"), sync_arg);
+  m.def("stem_backward", &stem_backward, py::arg("dp"), py::arg("x"), py::arg("code"), py::arg("weight"), py::arg("saved"), py::arg("work"),
+        sync_arg);
   m.def("stem_im2col", &stem_im2col);
-  m.def("conv1x1_bnstats", &conv1x1_bnstats);
+  m.def("conv1x1_bnstats", &conv1x1_bnstats, py::arg("x"), py::arg("weight"), py::arg("gsum"), sync_arg);
   m.def("normalize_nhwc", &normalize_nhwc);
   m.def("resample_normalize", &resample_normalize, py::arg("arena"), py::arg("n"), py::arg("out_h"), py::arg("out_w"), py::arg("max_rows"),
         py::arg("a"), py::arg("b"), py::arg("out_dtype"), py::arg("channels_last"));

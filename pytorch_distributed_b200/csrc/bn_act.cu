@@ -18,6 +18,7 @@
 
 #include <map>
 
+#include "bn_combine.cuh"
 #include "common.cuh"
 #include "host.h"
 
@@ -108,16 +109,9 @@ __global__ void __launch_bounds__(1024) combine_partials_kernel(const float* __r
   __shared__ float sm[32][33];
   const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
   const int i = blockIdx.x * 32 + tx;
-  float s = 0.f;
-  if (i < n)
-    for (int b = ty; b < nblocks; b += 32) s += part[(size_t)b * n + i];
-  sm[ty][tx] = s;
+  sm[ty][tx] = combine_slice(part, nblocks, n, i, ty);
   __syncthreads();
-  if (ty == 0 && i < n) {
-    float t = 0.f;
-    for (int k = 0; k < 32; ++k) t += sm[k][tx];
-    gsum[i] += t;
-  }
+  if (ty == 0 && i < n) gsum[i] += combine_fold(sm, tx);
 }
 
 void combine_partials(const float* part, int nblocks, int n, float* gsum, cudaStream_t st) {
@@ -165,16 +159,26 @@ __global__ void __launch_bounds__(kBnThreads) bn_stats_kernel(const T* __restric
   }
 }
 
+// Rows the statistics in gsum cover: this rank's M, or, synchronised (gsum = the global sums of a sync_bn_exchange work
+// slice), the global count stored right after them.
+template <bool SYNC>
+__device__ __forceinline__ int64_t stat_rows(const float* gsum, int C, int64_t M) {
+  if constexpr (SYNC) return *reinterpret_cast<const int64_t*>(gsum + 2 * C);
+  else return M;
+}
+
 // ------------------------------------------------------------------ forward: normalise (+res) (+relu)
-template <typename T, bool RELU, bool RES>
-__global__ void __launch_bounds__(kBnThreads) bn_apply_kernel(const T* __restrict__ x, const T* __restrict__ res, T* __restrict__ y,
-                                                              uint8_t* __restrict__ mask, const float* __restrict__ gsum,
-                                                              const void* __restrict__ w, const void* __restrict__ b, int wdt,
-                                                              float* __restrict__ running_mean, float* __restrict__ running_var,
-                                                              int64_t* __restrict__ num_batches_tracked, float* __restrict__ saved,
-                                                              int64_t M, int C, float eps, float momentum, int training) {
+#define BN_APPLY_PARAMS                                                                                                    \
+  const T *__restrict__ x, const T *__restrict__ res, T *__restrict__ y, uint8_t *__restrict__ mask,                      \
+      const float *__restrict__ gsum, const void *__restrict__ w, const void *__restrict__ b, int wdt,                    \
+      float *__restrict__ running_mean, float *__restrict__ running_var, int64_t *__restrict__ num_batches_tracked,       \
+      float *__restrict__ saved, int64_t M, int C, float eps, float momentum, int training
+#define BN_APPLY_ARGS x, res, y, mask, gsum, w, b, wdt, running_mean, running_var, num_batches_tracked, saved, M, C, eps, momentum, training
+template <typename T, bool RELU, bool RES, bool SYNC>
+__device__ __forceinline__ void bn_apply_body(BN_APPLY_PARAMS) {
   const RowMap m = row_map(C);
-  const float inv_m = 1.f / (float)M;
+  const int64_t N = stat_rows<SYNC>(gsum, C, M);
+  const float inv_m = 1.f / (float)N;
   if (training && num_batches_tracked && blockIdx.x == 0 && threadIdx.x == 0) *num_batches_tracked += 1;
   if (!m.active) return;
   for (int cg = m.cg0; cg < m.cgs; cg += m.tpr) {
@@ -197,7 +201,7 @@ __global__ void __launch_bounds__(kBnThreads) bn_apply_kernel(const T* __restric
         saved[c] = mean;
         saved[C + c] = invstd;
         if (running_mean) {
-          const float unbiased = M > 1 ? var * ((float)M / (float)(M - 1)) : var;
+          const float unbiased = N > 1 ? var * ((float)N / (float)(N - 1)) : var;
           running_mean[c] = (1.f - momentum) * running_mean[c] + momentum * mean;
           running_var[c] = (1.f - momentum) * running_var[c] + momentum * unbiased;
         }
@@ -245,6 +249,12 @@ __global__ void __launch_bounds__(kBnThreads) bn_apply_kernel(const T* __restric
     }
   }
 }
+template <typename T, bool RELU, bool RES>
+__global__ void __launch_bounds__(kBnThreads) bn_apply_kernel(BN_APPLY_PARAMS) { bn_apply_body<T, RELU, RES, false>(BN_APPLY_ARGS); }
+template <typename T, bool RELU, bool RES>
+__global__ void __launch_bounds__(kBnThreads) bn_apply_sync_kernel(BN_APPLY_PARAMS) { bn_apply_body<T, RELU, RES, true>(BN_APPLY_ARGS); }
+#undef BN_APPLY_PARAMS
+#undef BN_APPLY_ARGS
 
 // ------------------------------------------------------------------ backward: reductions
 // gsum[0:C] = sum dz ; gsum[C:2C] = sum dz * xhat   with dz = dy * relu_mask
@@ -309,15 +319,19 @@ __global__ void __launch_bounds__(kBnThreads) bn_bwd_reduce_kernel(const T* __re
 
 // ------------------------------------------------------------------ backward: apply
 // dx = gamma*invstd * (dz - mean(dz) - xhat * mean(dz*xhat)) ; dres = dz ; dgamma = sum dz*xhat ; dbeta = sum dz
-template <typename T, bool RELU, bool RES>
-__global__ void __launch_bounds__(kBnThreads) bn_bwd_apply_kernel(const T* __restrict__ dy, const uint8_t* __restrict__ mask,
-                                                                  const T* __restrict__ x, const float* __restrict__ saved,
-                                                                  const float* __restrict__ gsum, const void* __restrict__ w, int wdt,
-                                                                  T* __restrict__ dx, T* __restrict__ dres, void* __restrict__ dw,
-                                                                  void* __restrict__ db, int64_t M, int C) {
+// Synchronised: the means are over the global batch (global sums / global count), dgamma and dbeta stay this rank's sums
+// (gsum - 2C in the sync_bn_exchange work slice), so that averaging the gradients over the ranks gives what
+// torch.nn.SyncBatchNorm under DDP gives.
+#define BN_BWD_APPLY_PARAMS                                                                                                \
+  const T *__restrict__ dy, const uint8_t *__restrict__ mask, const T *__restrict__ x, const float *__restrict__ saved,    \
+      const float *__restrict__ gsum, const void *__restrict__ w, int wdt, T *__restrict__ dx, T *__restrict__ dres,      \
+      void *__restrict__ dw, void *__restrict__ db, int64_t M, int C
+#define BN_BWD_APPLY_ARGS dy, mask, x, saved, gsum, w, wdt, dx, dres, dw, db, M, C
+template <typename T, bool RELU, bool RES, bool SYNC>
+__device__ __forceinline__ void bn_bwd_apply_body(BN_BWD_APPLY_PARAMS) {
   const RowMap m = row_map(C);
   if (!m.active) return;
-  const float inv_m = 1.f / (float)M;
+  const float inv_m = 1.f / (float)stat_rows<SYNC>(gsum, C, M);
   for (int cg = m.cg0; cg < m.cgs; cg += m.tpr) {
     // dx = A*dz + B*x + D  with A = gamma*invstd, B = -A*invstd*mean(dz*xhat), D = -A*mean(dz) - B*mean
     float ka[8], kb[8], kd[8];
@@ -330,8 +344,13 @@ __global__ void __launch_bounds__(kBnThreads) bn_bwd_apply_kernel(const T* __res
       kb[k] = -ka[k] * invstd * sdzx * inv_m;
       kd[k] = -ka[k] * sdz * inv_m - kb[k] * mean;
       if (blockIdx.x == 0 && m.rlocal == 0) {
-        st_w(dw, wdt, c, sdzx);
-        st_w(db, wdt, c, sdz);
+        if constexpr (SYNC) {
+          st_w(dw, wdt, c, gsum[c - C]);          // local sum dz * xhat
+          st_w(db, wdt, c, gsum[c - 2 * C]);      // local sum dz
+        } else {
+          st_w(dw, wdt, c, sdzx);
+          st_w(db, wdt, c, sdz);
+        }
       }
     }
     const int64_t stride = (int64_t)gridDim.x * m.rpp;
@@ -380,6 +399,16 @@ __global__ void __launch_bounds__(kBnThreads) bn_bwd_apply_kernel(const T* __res
     }
   }
 }
+template <typename T, bool RELU, bool RES>
+__global__ void __launch_bounds__(kBnThreads) bn_bwd_apply_kernel(BN_BWD_APPLY_PARAMS) {
+  bn_bwd_apply_body<T, RELU, RES, false>(BN_BWD_APPLY_ARGS);
+}
+template <typename T, bool RELU, bool RES>
+__global__ void __launch_bounds__(kBnThreads) bn_bwd_apply_sync_kernel(BN_BWD_APPLY_PARAMS) {
+  bn_bwd_apply_body<T, RELU, RES, true>(BN_BWD_APPLY_ARGS);
+}
+#undef BN_BWD_APPLY_PARAMS
+#undef BN_BWD_APPLY_ARGS
 
 // ------------------------------------------------------------------ host side
 static int wdtype(const at::Tensor& t) {
@@ -443,7 +472,7 @@ static int apply_grid(const Geometry& g) {
 template <typename T>
 static void fwd_impl(const at::Tensor& x, const at::Tensor* res, at::Tensor& y, at::Tensor& mask, at::Tensor& work, at::Tensor& saved,
                      const at::Tensor& w, const at::Tensor& b, at::Tensor& rm, at::Tensor& rv, at::Tensor& nbt, bool training, float momentum,
-                     float eps, bool relu, bool stats_ready) {
+                     float eps, bool relu, bool stats_ready, const SyncBN* sync) {
   const Geometry g = geometry(x);
   cudaStream_t st = at::cuda::getCurrentCUDAStream();
   const T* xp = reinterpret_cast<const T*>(x.data_ptr());
@@ -456,7 +485,8 @@ static void fwd_impl(const at::Tensor& x, const at::Tensor* res, at::Tensor& y, 
     at::Tensor part = partials(x, grid, g.C);
     bn_stats_kernel<T><<<grid, kBnThreads, g.smem, st>>>(xp, part.data_ptr<float>(), g.M, g.C, rpb);
     C10_CUDA_KERNEL_LAUNCH_CHECK();
-    combine_partials(part.data_ptr<float>(), grid, 2 * g.C, wk, st);
+    if (sync) sync_bn_exchange(part.data_ptr<float>(), grid, g.C, g.M, wk, *sync, st);
+    else combine_partials(part.data_ptr<float>(), grid, 2 * g.C, wk, st);
   }
   const int grid = apply_grid(g);
   float* rmp = rm.defined() ? rm.data_ptr<float>() : nullptr;
@@ -465,20 +495,34 @@ static void fwd_impl(const at::Tensor& x, const at::Tensor* res, at::Tensor& y, 
   float* sv = saved.defined() ? saved.data_ptr<float>() : nullptr;
   uint8_t* mk = mask.defined() ? mask.data_ptr<uint8_t>() : nullptr;
   const int wdt = wdtype(w);
-#define APPLY(R, S) \
-  bn_apply_kernel<T, R, S><<<grid, kBnThreads, 0, st>>>(xp, rp, yp, mk, wk, w.data_ptr(), b.data_ptr(), wdt, rmp, rvp, nb, sv, g.M, g.C, eps, momentum, training ? 1 : 0)
-  if (relu) { if (res) APPLY(true, true); else APPLY(true, false); }
-  else      { if (res) APPLY(false, true); else APPLY(false, false); }
+#define APPLY(K, R, S) \
+  K<T, R, S><<<grid, kBnThreads, 0, st>>>(xp, rp, yp, mk, wk, w.data_ptr(), b.data_ptr(), wdt, rmp, rvp, nb, sv, g.M, g.C, eps, momentum, training ? 1 : 0)
+  if (sync) {                         // the apply reads the global sums and count
+    wk += 2 * g.C;
+    if (relu) { if (res) APPLY(bn_apply_sync_kernel, true, true); else APPLY(bn_apply_sync_kernel, true, false); }
+    else      { if (res) APPLY(bn_apply_sync_kernel, false, true); else APPLY(bn_apply_sync_kernel, false, false); }
+  } else {
+    if (relu) { if (res) APPLY(bn_apply_kernel, true, true); else APPLY(bn_apply_kernel, true, false); }
+    else      { if (res) APPLY(bn_apply_kernel, false, true); else APPLY(bn_apply_kernel, false, false); }
+  }
 #undef APPLY
   C10_CUDA_KERNEL_LAUNCH_CHECK();
+}
+
+// A synchronised call needs a training-mode work slice of the exchange layout (host.h: kSyncWork)
+static void check_sync_work(const SyncBN* sync, const at::Tensor& work, int64_t C) {
+  if (!sync) return;
+  TORCH_CHECK(work.defined() && work.scalar_type() == at::kFloat && work.numel() >= kSyncWork(C),
+              "synchronised BatchNorm needs a work slice of ", kSyncWork(C), " floats");
 }
 
 // returns {y, saved(mean|invstd), relu_mask}; `work` = zeroed float[2C] accumulator supplied by the caller
 std::vector<at::Tensor> bn_act_forward(const at::Tensor& x, const c10::optional<at::Tensor>& residual, const at::Tensor& weight,
                                        const at::Tensor& bias, at::Tensor running_mean, at::Tensor running_var,
                                        c10::optional<at::Tensor> num_batches_tracked, bool training, double momentum, double eps, bool relu,
-                                       bool need_mask, at::Tensor work, bool stats_ready) {
+                                       bool need_mask, at::Tensor work, bool stats_ready, const SyncBN* sync) {
   check_nhwc(x, "x");
+  TORCH_CHECK(!sync || training, "eval-mode BatchNorm is never synchronised");
   TORCH_CHECK(weight.scalar_type() == bias.scalar_type() && weight.is_contiguous() && bias.is_contiguous());
   if (running_mean.defined()) TORCH_CHECK(running_mean.scalar_type() == at::kFloat && running_var.scalar_type() == at::kFloat, "running stats must be fp32");
   TORCH_CHECK(training || running_mean.defined(), "eval mode needs running statistics");
@@ -500,11 +544,12 @@ std::vector<at::Tensor> bn_act_forward(const at::Tensor& x, const c10::optional<
     TORCH_CHECK(work.defined() && work.scalar_type() == at::kFloat && work.numel() >= 2 * C, "work buffer too small");
     saved = at::empty({2 * C}, x.options().dtype(at::kFloat));
   }
+  check_sync_work(sync, work, C);
   if (relu && need_mask) mask = at::empty({x.numel() / 8}, x.options().dtype(at::kByte));
   switch (x.scalar_type()) {
-    case at::kBFloat16: fwd_impl<__nv_bfloat16>(x, res, y, mask, work, saved, weight, bias, running_mean, running_var, nbt, training, (float)momentum, (float)eps, relu, stats_ready); break;
-    case at::kHalf: fwd_impl<__half>(x, res, y, mask, work, saved, weight, bias, running_mean, running_var, nbt, training, (float)momentum, (float)eps, relu, stats_ready); break;
-    case at::kFloat: fwd_impl<float>(x, res, y, mask, work, saved, weight, bias, running_mean, running_var, nbt, training, (float)momentum, (float)eps, relu, stats_ready); break;
+    case at::kBFloat16: fwd_impl<__nv_bfloat16>(x, res, y, mask, work, saved, weight, bias, running_mean, running_var, nbt, training, (float)momentum, (float)eps, relu, stats_ready, sync); break;
+    case at::kHalf: fwd_impl<__half>(x, res, y, mask, work, saved, weight, bias, running_mean, running_var, nbt, training, (float)momentum, (float)eps, relu, stats_ready, sync); break;
+    case at::kFloat: fwd_impl<float>(x, res, y, mask, work, saved, weight, bias, running_mean, running_var, nbt, training, (float)momentum, (float)eps, relu, stats_ready, sync); break;
     default: TORCH_CHECK(false, "unsupported activation dtype");
   }
   return {y, saved, mask};
@@ -512,7 +557,8 @@ std::vector<at::Tensor> bn_act_forward(const at::Tensor& x, const c10::optional<
 
 template <typename T>
 static void bwd_impl(const at::Tensor& dy, const at::Tensor& mask, const at::Tensor& x, const at::Tensor& saved, at::Tensor& work,
-                     const at::Tensor& w, at::Tensor& dx, at::Tensor& dres, at::Tensor& dw, at::Tensor& db, bool relu, bool write_res) {
+                     const at::Tensor& w, at::Tensor& dx, at::Tensor& dres, at::Tensor& dw, at::Tensor& db, bool relu, bool write_res,
+                     const SyncBN* sync) {
   const Geometry g = geometry(x);
   cudaStream_t st = at::cuda::getCurrentCUDAStream();
   const T* dyp = reinterpret_cast<const T*>(dy.data_ptr());
@@ -528,22 +574,30 @@ static void bwd_impl(const at::Tensor& dy, const at::Tensor& mask, const at::Ten
   if (relu) bn_bwd_reduce_kernel<T, true><<<rgrid, kBnThreads, g.smem, st>>>(dyp, mk, xp, sv, pp, g.M, g.C, rpb);
   else      bn_bwd_reduce_kernel<T, false><<<rgrid, kBnThreads, g.smem, st>>>(dyp, mk, xp, sv, pp, g.M, g.C, rpb);
   C10_CUDA_KERNEL_LAUNCH_CHECK();
-  combine_partials(pp, rgrid, 2 * g.C, wk, st);
   const int grid = apply_grid(g);
   T* dxp = reinterpret_cast<T*>(dx.data_ptr());
   T* drp = write_res ? reinterpret_cast<T*>(dres.data_ptr()) : nullptr;
   const int wdt = wdtype(w);
-#define BAPPLY(R, S) \
-  bn_bwd_apply_kernel<T, R, S><<<grid, kBnThreads, 0, st>>>(dyp, mk, xp, sv, wk, w.data_ptr(), wdt, dxp, drp, dw.data_ptr(), db.data_ptr(), g.M, g.C)
-  if (relu) { if (write_res) BAPPLY(true, true); else BAPPLY(true, false); }
-  else      { if (write_res) BAPPLY(false, true); else BAPPLY(false, false); }
+#define BAPPLY(K, R, S) \
+  K<T, R, S><<<grid, kBnThreads, 0, st>>>(dyp, mk, xp, sv, wk, w.data_ptr(), wdt, dxp, drp, dw.data_ptr(), db.data_ptr(), g.M, g.C)
+  if (sync) {
+    sync_bn_exchange(pp, rgrid, g.C, g.M, wk, *sync, st);
+    wk += 2 * g.C;
+    if (relu) { if (write_res) BAPPLY(bn_bwd_apply_sync_kernel, true, true); else BAPPLY(bn_bwd_apply_sync_kernel, true, false); }
+    else      { if (write_res) BAPPLY(bn_bwd_apply_sync_kernel, false, true); else BAPPLY(bn_bwd_apply_sync_kernel, false, false); }
+  } else {
+    combine_partials(pp, rgrid, 2 * g.C, wk, st);
+    if (relu) { if (write_res) BAPPLY(bn_bwd_apply_kernel, true, true); else BAPPLY(bn_bwd_apply_kernel, true, false); }
+    else      { if (write_res) BAPPLY(bn_bwd_apply_kernel, false, true); else BAPPLY(bn_bwd_apply_kernel, false, false); }
+  }
 #undef BAPPLY
   C10_CUDA_KERNEL_LAUNCH_CHECK();
 }
 
 // returns {dx, dres (undefined if !has_residual), dweight, dbias}
 std::vector<at::Tensor> bn_act_backward(const at::Tensor& dy_in, const at::Tensor& x, const c10::optional<at::Tensor>& mask_opt,
-                                        const at::Tensor& weight, const at::Tensor& saved, bool relu, bool has_residual, at::Tensor work) {
+                                        const at::Tensor& weight, const at::Tensor& saved, bool relu, bool has_residual, at::Tensor work,
+                                        const SyncBN* sync) {
   check_nhwc(x, "x");
   at::Tensor dy = dy_in.is_contiguous(at::MemoryFormat::ChannelsLast) ? dy_in : dy_in.contiguous(at::MemoryFormat::ChannelsLast);
   TORCH_CHECK(dy.scalar_type() == x.scalar_type() && dy.sizes() == x.sizes());
@@ -561,10 +615,11 @@ std::vector<at::Tensor> bn_act_backward(const at::Tensor& dy_in, const at::Tenso
   if (has_residual) dres = (!relu) ? dy : at::empty_like(x, x.options().memory_format(at::MemoryFormat::ChannelsLast));
   at::Tensor dw = at::empty_like(weight), db = at::empty_like(weight);
   const bool write_res = has_residual && relu;  // without ReLU the residual gradient IS dy: no copy
+  check_sync_work(sync, work, C);
   switch (x.scalar_type()) {
-    case at::kBFloat16: bwd_impl<__nv_bfloat16>(dy, mask, x, saved, work, weight, dx, dres, dw, db, relu, write_res); break;
-    case at::kHalf: bwd_impl<__half>(dy, mask, x, saved, work, weight, dx, dres, dw, db, relu, write_res); break;
-    case at::kFloat: bwd_impl<float>(dy, mask, x, saved, work, weight, dx, dres, dw, db, relu, write_res); break;
+    case at::kBFloat16: bwd_impl<__nv_bfloat16>(dy, mask, x, saved, work, weight, dx, dres, dw, db, relu, write_res, sync); break;
+    case at::kHalf: bwd_impl<__half>(dy, mask, x, saved, work, weight, dx, dres, dw, db, relu, write_res, sync); break;
+    case at::kFloat: bwd_impl<float>(dy, mask, x, saved, work, weight, dx, dres, dw, db, relu, write_res, sync); break;
     default: TORCH_CHECK(false, "unsupported activation dtype");
   }
   return {dx, dres, dw, db};
@@ -646,7 +701,8 @@ __global__ void __launch_bounds__(kBnThreads) bn_bwd_reduce_sum_kernel(const T* 
 
 template <typename T>
 static void bwd2_impl(const at::Tensor& dya, const at::Tensor& dyb, const at::Tensor& mask, const at::Tensor& x, const at::Tensor& saved,
-                      at::Tensor& work, const at::Tensor& w, at::Tensor& g_out, at::Tensor& dx, at::Tensor& dw, at::Tensor& db, bool relu) {
+                      at::Tensor& work, const at::Tensor& w, at::Tensor& g_out, at::Tensor& dx, at::Tensor& dw, at::Tensor& db, bool relu,
+                      const SyncBN* sync) {
   const Geometry g = geometry(x);
   cudaStream_t st = at::cuda::getCurrentCUDAStream();
   const T* ap = reinterpret_cast<const T*>(dya.data_ptr());
@@ -664,18 +720,25 @@ static void bwd2_impl(const at::Tensor& dya, const at::Tensor& dyb, const at::Te
   if (relu) bn_bwd_reduce_sum_kernel<T, true><<<rgrid, kBnThreads, g.smem, st>>>(ap, bp, mk, xp, sv, gp, pp, g.M, g.C, rpb);
   else      bn_bwd_reduce_sum_kernel<T, false><<<rgrid, kBnThreads, g.smem, st>>>(ap, bp, mk, xp, sv, gp, pp, g.M, g.C, rpb);
   C10_CUDA_KERNEL_LAUNCH_CHECK();
-  combine_partials(pp, rgrid, 2 * g.C, wk, st);
   // second pass: g already carries the mask, and it IS the residual gradient -> the plain (no ReLU, no dres) apply variant
-  bn_bwd_apply_kernel<T, false, false><<<apply_grid(g), kBnThreads, 0, st>>>(gp, nullptr, xp, sv, wk, w.data_ptr(), wdtype(w),
-                                                                           reinterpret_cast<T*>(dx.data_ptr()), nullptr, dw.data_ptr(),
-                                                                           db.data_ptr(), g.M, g.C);
+  if (sync) {
+    sync_bn_exchange(pp, rgrid, g.C, g.M, wk, *sync, st);
+    bn_bwd_apply_sync_kernel<T, false, false><<<apply_grid(g), kBnThreads, 0, st>>>(gp, nullptr, xp, sv, wk + 2 * g.C, w.data_ptr(), wdtype(w),
+                                                                                  reinterpret_cast<T*>(dx.data_ptr()), nullptr, dw.data_ptr(),
+                                                                                  db.data_ptr(), g.M, g.C);
+  } else {
+    combine_partials(pp, rgrid, 2 * g.C, wk, st);
+    bn_bwd_apply_kernel<T, false, false><<<apply_grid(g), kBnThreads, 0, st>>>(gp, nullptr, xp, sv, wk, w.data_ptr(), wdtype(w),
+                                                                             reinterpret_cast<T*>(dx.data_ptr()), nullptr, dw.data_ptr(),
+                                                                             db.data_ptr(), g.M, g.C);
+  }
   C10_CUDA_KERNEL_LAUNCH_CHECK();
 }
 
 // returns {dx, g = (dy_a + dy_b) * relu_mask (the residual gradient), dweight, dbias}
 std::vector<at::Tensor> bn_act_backward2(const at::Tensor& dy_a_in, const at::Tensor& dy_b_in, const at::Tensor& x,
                                          const c10::optional<at::Tensor>& mask_opt, const at::Tensor& weight, const at::Tensor& saved,
-                                         bool relu, at::Tensor work) {
+                                         bool relu, at::Tensor work, const SyncBN* sync) {
   check_nhwc(x, "x");
   const auto cl = at::MemoryFormat::ChannelsLast;
   at::Tensor dya = dy_a_in.is_contiguous(cl) ? dy_a_in : dy_a_in.contiguous(cl);
@@ -695,10 +758,11 @@ std::vector<at::Tensor> bn_act_backward2(const at::Tensor& dy_a_in, const at::Te
   at::Tensor g = at::empty_like(x, x.options().memory_format(cl));
   at::Tensor dx = at::empty_like(x, x.options().memory_format(cl));
   at::Tensor dw = at::empty_like(weight), db = at::empty_like(weight);
+  check_sync_work(sync, work, C);
   switch (x.scalar_type()) {
-    case at::kBFloat16: bwd2_impl<__nv_bfloat16>(dya, dyb, mask, x, saved, work, weight, g, dx, dw, db, relu); break;
-    case at::kHalf: bwd2_impl<__half>(dya, dyb, mask, x, saved, work, weight, g, dx, dw, db, relu); break;
-    case at::kFloat: bwd2_impl<float>(dya, dyb, mask, x, saved, work, weight, g, dx, dw, db, relu); break;
+    case at::kBFloat16: bwd2_impl<__nv_bfloat16>(dya, dyb, mask, x, saved, work, weight, g, dx, dw, db, relu, sync); break;
+    case at::kHalf: bwd2_impl<__half>(dya, dyb, mask, x, saved, work, weight, g, dx, dw, db, relu, sync); break;
+    case at::kFloat: bwd2_impl<float>(dya, dyb, mask, x, saved, work, weight, g, dx, dw, db, relu, sync); break;
     default: TORCH_CHECK(false, "unsupported activation dtype");
   }
   return {dx, g, dw, db};
@@ -740,17 +804,19 @@ __device__ __forceinline__ void stem_scale_shift(const float* gsum, const float*
   }
 }
 
-template <typename T>
-__global__ void __launch_bounds__(kBnThreads) stem_fwd_kernel(const T* __restrict__ x, T* __restrict__ y, uint2* __restrict__ code,
-                                                              const float* __restrict__ gsum, const void* __restrict__ w,
-                                                              const void* __restrict__ b, int wdt, float* __restrict__ running_mean,
-                                                              float* __restrict__ running_var, int64_t* __restrict__ nbt,
-                                                              float* __restrict__ saved, int64_t M, int N, int C, PoolGeom g, float eps,
-                                                              float momentum, int training) {
+#define STEM_FWD_PARAMS                                                                                                    \
+  const T *__restrict__ x, T *__restrict__ y, uint2 *__restrict__ code, const float *__restrict__ gsum,                   \
+      const void *__restrict__ w, const void *__restrict__ b, int wdt, float *__restrict__ running_mean,                  \
+      float *__restrict__ running_var, int64_t *__restrict__ nbt, float *__restrict__ saved, int64_t M, int N, int C,     \
+      PoolGeom g, float eps, float momentum, int training
+#define STEM_FWD_ARGS x, y, code, gsum, w, b, wdt, running_mean, running_var, nbt, saved, M, N, C, g, eps, momentum, training
+template <typename T, bool SYNC>
+__device__ __forceinline__ void stem_fwd_body(STEM_FWD_PARAMS) {
   const int cgs = C >> 3;
   const int cg = threadIdx.x % cgs;                 // host guarantees blockDim.x % cgs == 0
+  const int64_t rows = stat_rows<SYNC>(gsum, C, M);
   float sc[8], sh[8], mean[8], var[8];
-  stem_scale_shift(gsum, running_mean, running_var, w, b, wdt, cg, C, 1.f / (float)M, eps, training, sc, sh, mean, var);
+  stem_scale_shift(gsum, running_mean, running_var, w, b, wdt, cg, C, 1.f / (float)rows, eps, training, sc, sh, mean, var);
   if (training && blockIdx.x == 0 && threadIdx.x < cgs) {
     if (threadIdx.x == 0 && nbt) *nbt += 1;
 #pragma unroll
@@ -759,7 +825,7 @@ __global__ void __launch_bounds__(kBnThreads) stem_fwd_kernel(const T* __restric
       saved[c] = mean[k];
       saved[C + c] = rsqrtf(var[k] + eps);
       if (running_mean) {
-        const float unbiased = M > 1 ? var[k] * ((float)M / (float)(M - 1)) : var[k];
+        const float unbiased = rows > 1 ? var[k] * ((float)rows / (float)(rows - 1)) : var[k];
         running_mean[c] = (1.f - momentum) * running_mean[c] + momentum * mean[k];
         running_var[c] = (1.f - momentum) * running_var[c] + momentum * unbiased;
       }
@@ -804,6 +870,12 @@ __global__ void __launch_bounds__(kBnThreads) stem_fwd_kernel(const T* __restric
     }
   }
 }
+template <typename T>
+__global__ void __launch_bounds__(kBnThreads) stem_fwd_kernel(STEM_FWD_PARAMS) { stem_fwd_body<T, false>(STEM_FWD_ARGS); }
+template <typename T>
+__global__ void __launch_bounds__(kBnThreads) stem_fwd_sync_kernel(STEM_FWD_PARAMS) { stem_fwd_body<T, true>(STEM_FWD_ARGS); }
+#undef STEM_FWD_PARAMS
+#undef STEM_FWD_ARGS
 
 // dz (gradient w.r.t. the BN+ReLU output at one input position) = sum of the pooled gradients that selected it.
 // 16-bit dtypes stay packed: vcmpeq4 turns the 8 arg-max bytes into byte masks, PRMT widens them to 16-bit lane masks,
@@ -986,15 +1058,16 @@ __global__ void __launch_bounds__(kBnThreads, 4) stem_bwd_reduce_kernel(const T*
   cta_combine(m, 0, s, q, sm, part, C);
 }
 
-template <typename T>
-__global__ void __launch_bounds__(kBnThreads, 4) stem_bwd_apply_kernel(const T* __restrict__ dp, const uint2* __restrict__ code,
-                                                                    const T* __restrict__ x, const float* __restrict__ saved,
-                                                                    const float* __restrict__ gsum, const void* __restrict__ w, int wdt,
-                                                                    T* __restrict__ dx, void* __restrict__ dw, void* __restrict__ db,
-                                                                    int64_t M, int C, PoolGeom g, int rows_per_block) {
+#define STEM_BWD_APPLY_PARAMS                                                                                              \
+  const T *__restrict__ dp, const uint2 *__restrict__ code, const T *__restrict__ x, const float *__restrict__ saved,      \
+      const float *__restrict__ gsum, const void *__restrict__ w, int wdt, T *__restrict__ dx, void *__restrict__ dw,     \
+      void *__restrict__ db, int64_t M, int C, PoolGeom g, int rows_per_block
+#define STEM_BWD_APPLY_ARGS dp, code, x, saved, gsum, w, wdt, dx, dw, db, M, C, g, rows_per_block
+template <typename T, bool SYNC>
+__device__ __forceinline__ void stem_bwd_apply_body(STEM_BWD_APPLY_PARAMS) {
   const RowMap m = row_map(C);
   const int cg = m.cg0;
-  const float inv_m = 1.f / (float)M;
+  const float inv_m = 1.f / (float)stat_rows<SYNC>(gsum, C, M);
   float ka[8], kb[8], kd[8];
 #pragma unroll
   for (int k = 0; k < 8; ++k) {
@@ -1005,8 +1078,13 @@ __global__ void __launch_bounds__(kBnThreads, 4) stem_bwd_apply_kernel(const T* 
     kb[k] = -ka[k] * invstd * sdzx * inv_m;
     kd[k] = -ka[k] * sdz * inv_m - kb[k] * mean;
     if (blockIdx.x == 0 && m.rlocal == 0) {
-      st_w(dw, wdt, c, sdzx);
-      st_w(db, wdt, c, sdz);
+      if constexpr (SYNC) {                  // dgamma / dbeta: this rank's sums (see bn_bwd_apply_body)
+        st_w(dw, wdt, c, gsum[c - C]);
+        st_w(db, wdt, c, gsum[c - 2 * C]);
+      } else {
+        st_w(dw, wdt, c, sdzx);
+        st_w(db, wdt, c, sdz);
+      }
     }
   }
   const int QH = (g.H + 1) >> 1, QW = (g.W + 1) >> 1;
@@ -1034,6 +1112,16 @@ __global__ void __launch_bounds__(kBnThreads, 4) stem_bwd_apply_kernel(const T* 
     }
   }
 }
+template <typename T>
+__global__ void __launch_bounds__(kBnThreads, 4) stem_bwd_apply_kernel(STEM_BWD_APPLY_PARAMS) {
+  stem_bwd_apply_body<T, false>(STEM_BWD_APPLY_ARGS);
+}
+template <typename T>
+__global__ void __launch_bounds__(kBnThreads) stem_bwd_apply_sync_kernel(STEM_BWD_APPLY_PARAMS) {   // no spills at 4 CTAs/SM
+  stem_bwd_apply_body<T, true>(STEM_BWD_APPLY_ARGS);
+}
+#undef STEM_BWD_APPLY_PARAMS
+#undef STEM_BWD_APPLY_ARGS
 
 static PoolGeom pool_geom(const at::Tensor& x) {
   PoolGeom g;
@@ -1047,7 +1135,7 @@ static PoolGeom pool_geom(const at::Tensor& x) {
 template <typename T>
 static void stem_fwd_impl(const at::Tensor& x, at::Tensor& y, at::Tensor& code, at::Tensor& work, at::Tensor& saved, const at::Tensor& w,
                           const at::Tensor& b, at::Tensor& rm, at::Tensor& rv, at::Tensor& nbt, bool training, float momentum, float eps,
-                          bool stats_ready) {
+                          bool stats_ready, const SyncBN* sync) {
   const Geometry g = geometry(x);
   const PoolGeom pg = pool_geom(x);
   cudaStream_t st = at::cuda::getCurrentCUDAStream();
@@ -1059,18 +1147,19 @@ static void stem_fwd_impl(const at::Tensor& x, at::Tensor& y, at::Tensor& code, 
     at::Tensor part = partials(x, grid, g.C);
     bn_stats_kernel<T><<<grid, kBnThreads, g.smem, st>>>(xp, part.data_ptr<float>(), g.M, g.C, rpb);
     C10_CUDA_KERNEL_LAUNCH_CHECK();
-    combine_partials(part.data_ptr<float>(), grid, 2 * g.C, wk, st);
+    if (sync) sync_bn_exchange(part.data_ptr<float>(), grid, g.C, g.M, wk, *sync, st);
+    else combine_partials(part.data_ptr<float>(), grid, 2 * g.C, wk, st);
   }
   const int cgs = g.C / 8;
   const int64_t total = x.size(0) * pg.OH * pg.OW;
   const int ppb = kBnThreads / cgs;
   const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((total + ppb - 1) / ppb, (int64_t)g.sms * 16));
-  stem_fwd_kernel<T><<<grid, kBnThreads, 0, st>>>(xp, reinterpret_cast<T*>(y.data_ptr()),
-                                                 code.defined() ? reinterpret_cast<uint2*>(code.data_ptr()) : nullptr, wk, w.data_ptr(),
-                                                 b.data_ptr(), wdtype(w), rm.defined() ? rm.data_ptr<float>() : nullptr,
-                                                 rv.defined() ? rv.data_ptr<float>() : nullptr, nbt.defined() ? nbt.data_ptr<int64_t>() : nullptr,
-                                                 saved.defined() ? saved.data_ptr<float>() : nullptr, g.M, (int)x.size(0), g.C, pg, eps, momentum,
-                                                 training ? 1 : 0);
+  auto kernel = sync ? stem_fwd_sync_kernel<T> : stem_fwd_kernel<T>;
+  kernel<<<grid, kBnThreads, 0, st>>>(xp, reinterpret_cast<T*>(y.data_ptr()), code.defined() ? reinterpret_cast<uint2*>(code.data_ptr()) : nullptr,
+                                      sync ? wk + 2 * g.C : wk, w.data_ptr(), b.data_ptr(), wdtype(w), rm.defined() ? rm.data_ptr<float>() : nullptr,
+                                      rv.defined() ? rv.data_ptr<float>() : nullptr, nbt.defined() ? nbt.data_ptr<int64_t>() : nullptr,
+                                      saved.defined() ? saved.data_ptr<float>() : nullptr, g.M, (int)x.size(0), g.C, pg, eps, momentum,
+                                      training ? 1 : 0);
   C10_CUDA_KERNEL_LAUNCH_CHECK();
 }
 
@@ -1078,8 +1167,9 @@ static void stem_fwd_impl(const at::Tensor& x, at::Tensor& y, at::Tensor& code, 
 static std::vector<at::Tensor> stem_forward_common(const at::Tensor& x, const at::Tensor& weight, const at::Tensor& bias,
                                                    at::Tensor running_mean, at::Tensor running_var,
                                                    c10::optional<at::Tensor> num_batches_tracked, bool training, double momentum, double eps,
-                                                   bool need_code, at::Tensor work, bool stats_ready) {
+                                                   bool need_code, at::Tensor work, bool stats_ready, const SyncBN* sync) {
   check_nhwc(x, "x");
+  TORCH_CHECK(!sync || training, "eval-mode BatchNorm is never synchronised");
   const int C = (int)x.size(1);
   TORCH_CHECK(C % 8 == 0 && kBnThreads % (C / 8) == 0, "fused stem needs C/8 to divide ", kBnThreads);
   TORCH_CHECK(x.numel() / C < (int64_t)1 << 30, "fused stem: too many pixels for 32-bit indexing");
@@ -1094,10 +1184,11 @@ static std::vector<at::Tensor> stem_forward_common(const at::Tensor& x, const at
     saved = at::empty({2 * C}, x.options().dtype(at::kFloat));
   }
   if (need_code) code = at::empty({y.numel()}, x.options().dtype(at::kByte));
+  check_sync_work(sync, work, C);
   switch (x.scalar_type()) {
-    case at::kBFloat16: stem_fwd_impl<__nv_bfloat16>(x, y, code, work, saved, weight, bias, running_mean, running_var, nbt, training, (float)momentum, (float)eps, stats_ready); break;
-    case at::kHalf: stem_fwd_impl<__half>(x, y, code, work, saved, weight, bias, running_mean, running_var, nbt, training, (float)momentum, (float)eps, stats_ready); break;
-    case at::kFloat: stem_fwd_impl<float>(x, y, code, work, saved, weight, bias, running_mean, running_var, nbt, training, (float)momentum, (float)eps, stats_ready); break;
+    case at::kBFloat16: stem_fwd_impl<__nv_bfloat16>(x, y, code, work, saved, weight, bias, running_mean, running_var, nbt, training, (float)momentum, (float)eps, stats_ready, sync); break;
+    case at::kHalf: stem_fwd_impl<__half>(x, y, code, work, saved, weight, bias, running_mean, running_var, nbt, training, (float)momentum, (float)eps, stats_ready, sync); break;
+    case at::kFloat: stem_fwd_impl<float>(x, y, code, work, saved, weight, bias, running_mean, running_var, nbt, training, (float)momentum, (float)eps, stats_ready, sync); break;
     default: TORCH_CHECK(false, "unsupported activation dtype");
   }
   return {y, saved, code};
@@ -1105,19 +1196,22 @@ static std::vector<at::Tensor> stem_forward_common(const at::Tensor& x, const at
 
 std::vector<at::Tensor> stem_forward(const at::Tensor& x, const at::Tensor& weight, const at::Tensor& bias, at::Tensor running_mean,
                                      at::Tensor running_var, c10::optional<at::Tensor> num_batches_tracked, bool training, double momentum,
-                                     double eps, bool need_code, at::Tensor work) {
-  return stem_forward_common(x, weight, bias, running_mean, running_var, num_batches_tracked, training, momentum, eps, need_code, work, false);
+                                     double eps, bool need_code, at::Tensor work, const SyncBN* sync) {
+  return stem_forward_common(x, weight, bias, running_mean, running_var, num_batches_tracked, training, momentum, eps, need_code, work, false,
+                             sync);
 }
-// same, with the per-channel sum / sum of squares of x already accumulated in work[0:2C] (stem convolution run as a GEMM)
+// same, with the per-channel sum / sum of squares of x already accumulated in work[0:2C] (stem convolution run as a GEMM;
+// synchronised: the GEMM's exchange already filled the whole work slice)
 std::vector<at::Tensor> stem_forward_pre(const at::Tensor& x, const at::Tensor& weight, const at::Tensor& bias, at::Tensor running_mean,
                                          at::Tensor running_var, c10::optional<at::Tensor> num_batches_tracked, bool training, double momentum,
-                                         double eps, bool need_code, at::Tensor work) {
-  return stem_forward_common(x, weight, bias, running_mean, running_var, num_batches_tracked, training, momentum, eps, need_code, work, true);
+                                         double eps, bool need_code, at::Tensor work, const SyncBN* sync) {
+  return stem_forward_common(x, weight, bias, running_mean, running_var, num_batches_tracked, training, momentum, eps, need_code, work, true,
+                             sync);
 }
 
 template <typename T>
 static void stem_bwd_impl(const at::Tensor& dp, const at::Tensor& code, const at::Tensor& x, const at::Tensor& saved, at::Tensor& work,
-                          const at::Tensor& w, at::Tensor& dx, at::Tensor& dw, at::Tensor& db) {
+                          const at::Tensor& w, at::Tensor& dx, at::Tensor& dw, at::Tensor& db, const SyncBN* sync) {
   const Geometry g = geometry(x);
   const PoolGeom pg = pool_geom(x);
   cudaStream_t st = at::cuda::getCurrentCUDAStream();
@@ -1130,27 +1224,35 @@ static void stem_bwd_impl(const at::Tensor& dp, const at::Tensor& code, const at
   at::Tensor part = partials(x, grid, g.C);
   stem_bwd_reduce_kernel<T><<<grid, kBnThreads, g.smem, st>>>(dpp, cp, xp, saved.data_ptr<float>(), part.data_ptr<float>(), g.M, g.C, pg, rpb);
   C10_CUDA_KERNEL_LAUNCH_CHECK();
-  combine_partials(part.data_ptr<float>(), grid, 2 * g.C, work.data_ptr<float>(), st);
-  stem_bwd_apply_kernel<T><<<grid, kBnThreads, 0, st>>>(dpp, cp, xp, saved.data_ptr<float>(), work.data_ptr<float>(), w.data_ptr(), wdtype(w),
-                                                       reinterpret_cast<T*>(dx.data_ptr()), dw.data_ptr(), db.data_ptr(), g.M, g.C, pg, rpb);
+  if (sync) {
+    sync_bn_exchange(part.data_ptr<float>(), grid, g.C, g.M, work.data_ptr<float>(), *sync, st);
+    stem_bwd_apply_sync_kernel<T><<<grid, kBnThreads, 0, st>>>(dpp, cp, xp, saved.data_ptr<float>(), work.data_ptr<float>() + 2 * g.C, w.data_ptr(),
+                                                              wdtype(w), reinterpret_cast<T*>(dx.data_ptr()), dw.data_ptr(), db.data_ptr(), g.M,
+                                                              g.C, pg, rpb);
+  } else {
+    combine_partials(part.data_ptr<float>(), grid, 2 * g.C, work.data_ptr<float>(), st);
+    stem_bwd_apply_kernel<T><<<grid, kBnThreads, 0, st>>>(dpp, cp, xp, saved.data_ptr<float>(), work.data_ptr<float>(), w.data_ptr(), wdtype(w),
+                                                         reinterpret_cast<T*>(dx.data_ptr()), dw.data_ptr(), db.data_ptr(), g.M, g.C, pg, rpb);
+  }
   C10_CUDA_KERNEL_LAUNCH_CHECK();
 }
 
 // returns {dx, dweight, dbias}
 std::vector<at::Tensor> stem_backward(const at::Tensor& dp_in, const at::Tensor& x, const at::Tensor& code, const at::Tensor& weight,
-                                      const at::Tensor& saved, at::Tensor work) {
+                                      const at::Tensor& saved, at::Tensor work, const SyncBN* sync) {
   check_nhwc(x, "x");
   at::Tensor dp = dp_in.is_contiguous(at::MemoryFormat::ChannelsLast) ? dp_in : dp_in.contiguous(at::MemoryFormat::ChannelsLast);
   const int C = (int)x.size(1);
   TORCH_CHECK(dp.scalar_type() == x.scalar_type() && dp.size(1) == C && code.scalar_type() == at::kByte && code.numel() == dp.numel());
   TORCH_CHECK(work.defined() && work.numel() >= 2 * C, "work buffer too small");
+  check_sync_work(sync, work, C);
   c10::cuda::CUDAGuard guard(x.device());
   at::Tensor dx = at::empty_like(x, x.options().memory_format(at::MemoryFormat::ChannelsLast));
   at::Tensor dw = at::empty_like(weight), db = at::empty_like(weight);
   switch (x.scalar_type()) {
-    case at::kBFloat16: stem_bwd_impl<__nv_bfloat16>(dp, code, x, saved, work, weight, dx, dw, db); break;
-    case at::kHalf: stem_bwd_impl<__half>(dp, code, x, saved, work, weight, dx, dw, db); break;
-    case at::kFloat: stem_bwd_impl<float>(dp, code, x, saved, work, weight, dx, dw, db); break;
+    case at::kBFloat16: stem_bwd_impl<__nv_bfloat16>(dp, code, x, saved, work, weight, dx, dw, db, sync); break;
+    case at::kHalf: stem_bwd_impl<__half>(dp, code, x, saved, work, weight, dx, dw, db, sync); break;
+    case at::kFloat: stem_bwd_impl<float>(dp, code, x, saved, work, weight, dx, dw, db, sync); break;
     default: TORCH_CHECK(false, "unsupported activation dtype");
   }
   return {dx, dw, db};

@@ -33,4 +33,19 @@ struct CommCtx {
 
 enum DType : int { kF32 = 0, kBF16 = 1, kF16 = 2 };
 
+// Synchronised BatchNorm (sync_bn.cu).  Exchange area, at the same arena offset on every rank:
+//   uint2 words[2 parities][kMaxWorld source ranks][kSyncBnSlotWords] of {payload bits, sequence}
+// A slot carries one rank's [2C] local sums followed by its row count as two 32-bit halves.
+constexpr int kSyncBnMaxC = 8192;
+constexpr int kSyncBnSlotWords = 2 * kSyncBnMaxC + 2;
+constexpr int64_t kSyncBnAreaBytes = (int64_t)2 * kMaxWorld * kSyncBnSlotWords * 8;
+
+// What a synchronised BatchNorm call needs to reach its peers.  `calls`: this handle's local [kMaxBlocks] call counters
+// (all entries advance together, one per exchange).
+struct SyncBN {
+  CommCtx ctx;
+  int64_t xoff;        // arena byte offset of the exchange area
+  uint32_t* calls;
+};
+
 }  // namespace ptd

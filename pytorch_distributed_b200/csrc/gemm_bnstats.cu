@@ -290,7 +290,7 @@ static CUtensorMap make_map(CUtensorMapDataType dtype, const void* ptr, int64_t 
 }
 
 template <typename T, int BLOCK_N>
-static void launch_gemm(const at::Tensor& a, const at::Tensor& b, at::Tensor& c, at::Tensor& gsum, int M, int N, int K) {
+static void launch_gemm(const at::Tensor& a, const at::Tensor& b, at::Tensor& c, at::Tensor& gsum, int M, int N, int K, const SyncBN* sync) {
   constexpr int smem = GemmCfg<BLOCK_N>::kSmem;
   static bool configured[64] = {};                 // the attribute is per device (DataParallel drives several from one process)
   const int dev = a.get_device();
@@ -310,20 +310,22 @@ static void launch_gemm(const at::Tensor& a, const at::Tensor& b, at::Tensor& c,
   at::Tensor part = at::empty({ctas_per_n, 2 * N}, gsum.options());
   gemm_bnstats_kernel<T, BLOCK_N><<<grid, kGemmThreads, smem, st>>>(ma, mb, mc, part.data_ptr<float>(), N, K, m_tiles, n_tiles, ctas_per_n);
   C10_CUDA_KERNEL_LAUNCH_CHECK();
-  combine_partials(part.data_ptr<float>(), ctas_per_n, 2 * N, gsum.data_ptr<float>(), st);
+  if (sync) sync_bn_exchange(part.data_ptr<float>(), ctas_per_n, N, M, gsum.data_ptr<float>(), *sync, st);
+  else combine_partials(part.data_ptr<float>(), ctas_per_n, 2 * N, gsum.data_ptr<float>(), st);
 }
 
 template <typename T>
-static void launch_gemm_for(const at::Tensor& a, const at::Tensor& b, at::Tensor& c, at::Tensor& gsum, int M, int N, int K) {
+static void launch_gemm_for(const at::Tensor& a, const at::Tensor& b, at::Tensor& c, at::Tensor& gsum, int M, int N, int K, const SyncBN* sync) {
   static const int max_bn = getenv("PTD_GEMM_BLOCK_N") ? atoi(getenv("PTD_GEMM_BLOCK_N")) : 256;
-  if (N % 256 == 0 && max_bn >= 256) launch_gemm<T, 256>(a, b, c, gsum, M, N, K);
-  else if (N % 128 == 0 && max_bn >= 128) launch_gemm<T, 128>(a, b, c, gsum, M, N, K);
-  else launch_gemm<T, 64>(a, b, c, gsum, M, N, K);
+  if (N % 256 == 0 && max_bn >= 256) launch_gemm<T, 256>(a, b, c, gsum, M, N, K, sync);
+  else if (N % 128 == 0 && max_bn >= 128) launch_gemm<T, 128>(a, b, c, gsum, M, N, K, sync);
+  else launch_gemm<T, 64>(a, b, c, gsum, M, N, K, sync);
 }
 
 // x: [B, K, H, W] channels_last bf16 or fp16; weight: [N, K, 1, 1] of x's dtype (any dense layout); gsum: zeroed float[2N].
 // returns y [B, N, H, W] channels_last in x's dtype; gsum accumulates the per-channel sum and sum of squares of y.
-at::Tensor conv1x1_bnstats(const at::Tensor& x, const at::Tensor& weight, at::Tensor gsum) {
+// sync: gsum is a synchronised work slice (host.h kSyncWork) and the epilogue partials go through the cross-rank exchange.
+at::Tensor conv1x1_bnstats(const at::Tensor& x, const at::Tensor& weight, at::Tensor gsum, const SyncBN* sync) {
   const bool is16 = x.scalar_type() == at::kBFloat16 || x.scalar_type() == at::kHalf;
   TORCH_CHECK(x.is_cuda() && x.dim() == 4 && is16 && x.is_contiguous(at::MemoryFormat::ChannelsLast),
               "conv1x1_bnstats: x must be a channels_last bf16 or fp16 CUDA tensor");
@@ -332,14 +334,14 @@ at::Tensor conv1x1_bnstats(const at::Tensor& x, const at::Tensor& weight, at::Te
   const int64_t M64 = x.size(0) * x.size(2) * x.size(3);
   const int K = (int)x.size(1), N = (int)weight.size(0);
   TORCH_CHECK(weight.size(1) == K && K % kBlockK == 0 && N % 64 == 0 && M64 < (int64_t)1 << 31, "conv1x1_bnstats: unsupported shape");
-  TORCH_CHECK(gsum.scalar_type() == at::kFloat && gsum.numel() >= 2 * N && gsum.is_contiguous());
+  TORCH_CHECK(gsum.scalar_type() == at::kFloat && gsum.numel() >= (sync ? kSyncWork(N) : 2 * N) && gsum.is_contiguous());
   TORCH_CHECK((reinterpret_cast<uintptr_t>(x.data_ptr()) & 15) == 0, "x must be 16-byte aligned");
   c10::cuda::CUDAGuard guard(x.device());
   at::Tensor w2 = weight.reshape({N, K}).contiguous();       // [N, K] K-major (a view for both NCHW and NHWC 1x1 weights)
   at::Tensor y = at::empty({x.size(0), N, x.size(2), x.size(3)}, x.options().memory_format(at::MemoryFormat::ChannelsLast));
   const int M = (int)M64;
-  if (x.scalar_type() == at::kHalf) launch_gemm_for<__half>(x, w2, y, gsum, M, N, K);
-  else launch_gemm_for<__nv_bfloat16>(x, w2, y, gsum, M, N, K);
+  if (x.scalar_type() == at::kHalf) launch_gemm_for<__half>(x, w2, y, gsum, M, N, K, sync);
+  else launch_gemm_for<__nv_bfloat16>(x, w2, y, gsum, M, N, K, sync);
   return y;
 }
 

@@ -45,27 +45,38 @@ void amp_update_scale(at::Tensor scale, at::Tensor growth_tracker, at::Tensor fo
 // ---- bn_act.cu
 // gsum[0:n] += the rows part[0:nblocks][0:n] summed in a fixed order (deterministic cross-CTA reduction)
 void combine_partials(const float* part, int nblocks, int n, float* gsum, cudaStream_t st);
+// The entry points below take `sync` (nullptr: this rank alone).  With a handle, `work` is the synchronised layout
+// float[kSyncWork(C)] = [local 2C sums | global 2C sums | global row count (int64)] instead of the plain [2C] sums.
 std::vector<at::Tensor> bn_act_forward(const at::Tensor& x, const c10::optional<at::Tensor>& residual, const at::Tensor& weight,
                                        const at::Tensor& bias, at::Tensor running_mean, at::Tensor running_var,
                                        c10::optional<at::Tensor> num_batches_tracked, bool training, double momentum, double eps, bool relu,
-                                       bool need_mask, at::Tensor work, bool stats_ready);
+                                       bool need_mask, at::Tensor work, bool stats_ready, const SyncBN* sync);
 std::vector<at::Tensor> bn_act_backward(const at::Tensor& dy, const at::Tensor& x, const c10::optional<at::Tensor>& mask,
-                                        const at::Tensor& weight, const at::Tensor& saved, bool relu, bool has_residual, at::Tensor work);
+                                        const at::Tensor& weight, const at::Tensor& saved, bool relu, bool has_residual, at::Tensor work,
+                                        const SyncBN* sync);
 std::vector<at::Tensor> bn_act_backward2(const at::Tensor& dy_a, const at::Tensor& dy_b, const at::Tensor& x,
                                          const c10::optional<at::Tensor>& mask, const at::Tensor& weight, const at::Tensor& saved, bool relu,
-                                         at::Tensor work);
+                                         at::Tensor work, const SyncBN* sync);
 
 std::vector<at::Tensor> stem_forward(const at::Tensor& x, const at::Tensor& weight, const at::Tensor& bias, at::Tensor running_mean,
                                      at::Tensor running_var, c10::optional<at::Tensor> num_batches_tracked, bool training, double momentum,
-                                     double eps, bool need_code, at::Tensor work);
+                                     double eps, bool need_code, at::Tensor work, const SyncBN* sync);
 std::vector<at::Tensor> stem_forward_pre(const at::Tensor& x, const at::Tensor& weight, const at::Tensor& bias, at::Tensor running_mean,
                                          at::Tensor running_var, c10::optional<at::Tensor> num_batches_tracked, bool training, double momentum,
-                                         double eps, bool need_code, at::Tensor work);
+                                         double eps, bool need_code, at::Tensor work, const SyncBN* sync);
 std::vector<at::Tensor> stem_backward(const at::Tensor& dp, const at::Tensor& x, const at::Tensor& code, const at::Tensor& weight,
-                                      const at::Tensor& saved, at::Tensor work);
+                                      const at::Tensor& saved, at::Tensor work, const SyncBN* sync);
+
+// ---- sync_bn.cu
+// floats of a synchronised work slice for C channels (the int64 count stays 8-byte aligned: C % 8 == 0)
+constexpr int64_t kSyncWork(int64_t C) { return 4 * C + 4; }
+// Replaces combine_partials for a synchronised layer: work[0:2C] += the fixed-order combine of part (this rank's sums),
+// then every rank publishes them with its row count and work[2C:4C] / work[4C:4C+2] receive the rank-order global sums
+// and the global count.
+void sync_bn_exchange(const float* part, int nblocks, int C, int64_t rows, float* work, const SyncBN& s, cudaStream_t st);
 
 // ---- gemm_bnstats.cu (wgmma / TMA)
-at::Tensor conv1x1_bnstats(const at::Tensor& x, const at::Tensor& weight, at::Tensor gsum);
+at::Tensor conv1x1_bnstats(const at::Tensor& x, const at::Tensor& weight, at::Tensor gsum, const SyncBN* sync);
 
 // ---- stem_conv.cu
 at::Tensor stem_im2col(const at::Tensor& x);

@@ -494,6 +494,24 @@ STRATEGIES = {
 }
 
 
+def apply_sync_bn(model, args, st, device):
+    """``--sync-bn``: every BatchNorm layer becomes a synchronised one (``models.resnet.convert_sync_batchnorm``) before the
+    strategy casts and wraps the model."""
+    if not getattr(args, "sync_bn", False):
+        return model
+    if not st.distributed:
+        raise ValueError("--sync-bn needs one process per GPU; like torch.nn.SyncBatchNorm it does not support DataParallel")
+    kind = st.comm_kind(args, device)
+    if args.cuda_graph and kind != "fused":
+        raise ValueError("--sync-bn with --comm %s synchronises BatchNorm through torch.distributed, which a CUDA graph cannot "
+                         "capture; use --comm fused or drop --cuda-graph" % kind)
+    if args.cuda_graph and (args.fused_bn is False or args.channels_last is False):
+        raise ValueError("--sync-bn with --no-fused-bn / --no-channels-last synchronises BatchNorm through torch.distributed, "
+                         "which a CUDA graph cannot capture; drop --cuda-graph")
+    from .models.resnet import convert_sync_batchnorm
+    return convert_sync_batchnorm(model)
+
+
 # ====================================================================== the worker
 def main_worker(local_rank: int, nprocs: int, args, strategy: Optional[Strategy] = None):
     """/root/reference/distributed.py:129-225 (shared by every entrypoint)."""
@@ -505,6 +523,7 @@ def main_worker(local_rank: int, nprocs: int, args, strategy: Optional[Strategy]
     world = st.world() if st.distributed else 1
 
     model = create_model(args.arch, pretrained=args.pretrained, num_classes=args.num_classes, fused_bn=args.fused_bn)
+    model = apply_sync_bn(model, args, st, device)
     # per-process batch: "-b" is the total over the node (reference :146); DataParallel keeps the full batch (:166)
     args.total_batch_size = args.batch_size
     if st.shard_batch:

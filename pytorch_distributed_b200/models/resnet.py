@@ -54,7 +54,87 @@ class BNAct(nn.BatchNorm2d):
         nbt = self.num_batches_tracked if (self.training and self.track_running_stats) else None   # bumped inside the kernel
         return bn_act(x, self.weight, self.bias, self.running_mean, self.running_var, residual=residual, relu=self.relu,
                       training=training, momentum=0.1 if self.momentum is None else self.momentum, eps=self.eps, fused=self.fused,
-                      num_batches_tracked=nbt, split=split)
+                      num_batches_tracked=nbt, split=split, sync=self.sync_context())
+
+    def sync_context(self):
+        """The ``sync=`` handle of this layer's training-mode statistics: None (per-rank statistics)."""
+        return None
+
+
+def check_process_group(process_group) -> None:
+    """Synchronised BatchNorm spans the whole world: a subgroup is rejected (as apex DDP rejects its unsupported arguments)."""
+    import torch.distributed as dist
+    if process_group is None or (dist.is_available() and dist.is_initialized() and process_group is dist.group.WORLD):
+        return
+    if dist.is_available() and dist.is_initialized() and dist.get_world_size(process_group) == dist.get_world_size():
+        return
+    raise NotImplementedError("process_group: synchronised BatchNorm over a subgroup of the ranks is not supported; "
+                              "pass None (the whole world)")
+
+
+class SyncBNAct(BNAct):
+    """``BNAct`` whose training-mode statistics cover the global batch of all data-parallel ranks, with the semantics of
+    ``torch.nn.SyncBatchNorm``: mean / variance of the concatenated batch, running variance with the global unbiased
+    factor, input gradients through the global sums, weight / bias gradients from this rank's sums (the DDP average
+    then matches torch).  Eval mode and a world of 1 are plain ``BNAct``.
+
+    The layer binds to the process's communicator (``utils.dist_ops.set_default_communicator``, registered by this
+    package's DDP, apex DDP and ``hvd.init``) at its first training forward with world > 1.  With the fused communicator
+    the statistics are exchanged inside the fused BatchNorm kernels (``csrc/sync_bn.cu``); layers those kernels cannot
+    take, and other communicators, run ``torch.nn.SyncBatchNorm``'s autograd function over the process group."""
+
+    def __init__(self, num_features, eps=1e-5, momentum=0.1, affine=True, track_running_stats=True, process_group=None, relu=False,
+                 fused=None, **kw):
+        check_process_group(process_group)
+        super().__init__(num_features, relu=relu, fused=fused, eps=eps, momentum=momentum, affine=affine,
+                         track_running_stats=track_running_stats, **kw)
+        self._sync = None
+
+    def sync_context(self):
+        if not self.training:          # eval mode never synchronises (torch: need_sync = bn_training and self.training)
+            return None
+        if self._sync is None:
+            import torch.distributed as dist
+            if not (dist.is_available() and dist.is_initialized()) or dist.get_world_size() == 1:
+                return None
+            from ..ops.sync_bn import SyncContext
+            from ..utils.dist_ops import default_communicator
+            comm = default_communicator()
+            if comm is None:
+                raise RuntimeError("SyncBatchNorm: no communicator is registered for this process; wrap the model in this "
+                                   "package's DistributedDataParallel (or apex DDP, or call hvd.init()) before the first "
+                                   "training forward, or call utils.dist_ops.set_default_communicator(comm)")
+            self._sync = SyncContext.for_communicator(comm)
+        return self._sync if self._sync.world > 1 else None
+
+    @classmethod
+    def convert_sync_batchnorm(cls, module, process_group=None):
+        return convert_sync_batchnorm(module, process_group)
+
+
+def _to_sync(bn: nn.modules.batchnorm._BatchNorm) -> SyncBNAct:
+    new = SyncBNAct(bn.num_features, eps=bn.eps, momentum=bn.momentum, affine=bn.affine, track_running_stats=bn.track_running_stats,
+                    relu=getattr(bn, "relu", False), fused=getattr(bn, "fused", None))
+    new.training = bn.training
+    if bn.affine:                      # the very same Parameter objects: optimizers, DDP hooks and state_dict keys stay valid
+        new.weight, new.bias = bn.weight, bn.bias
+    for name in ("running_mean", "running_var", "num_batches_tracked"):
+        new._buffers[name] = bn._buffers.get(name)
+    return new
+
+
+def convert_sync_batchnorm(module: nn.Module, process_group=None) -> nn.Module:
+    """Every ``nn.BatchNorm2d`` (including ``BNAct``, keeping its ReLU) and ``torch.nn.SyncBatchNorm`` of ``module`` becomes a
+    :class:`SyncBNAct` sharing its Parameter and buffer objects; returns the converted module (``module`` itself unless it
+    is a BatchNorm layer), like ``torch.nn.SyncBatchNorm.convert_sync_batchnorm``."""
+    check_process_group(process_group)
+    if isinstance(module, (nn.BatchNorm2d, nn.SyncBatchNorm)) and not isinstance(module, SyncBNAct):
+        return _to_sync(module)
+    for name, child in module.named_children():
+        new = convert_sync_batchnorm(child, process_group)
+        if new is not child:
+            setattr(module, name, new)
+    return module
 
 
 def _conv3x3(cin, cout, stride=1, groups=1, dilation=1):
@@ -164,15 +244,16 @@ class ResNet(nn.Module):
         if self.training:
             begin_step(x.device)      # recycle the BN accumulator workspace: one memset per step
         bn = self.bn1
+        sync = bn.sync_context()
         if STEM_GEMM and bn.training and torch.is_grad_enabled() and bn.fused is not False and (
-                can_use_stem_gemm(x, self.conv1) or bn.fused == "emulate"):
+                (can_use_stem_gemm(x, self.conv1) and (sync is None or sync.native is not None)) or bn.fused == "emulate"):
             x = stem_conv_bn_relu_maxpool(x, self.conv1, bn, emulate=bn.fused == "emulate")
             x = self.layer4(self.layer3(self.layer2(self.layer1(x))))
             return self.fc(torch.flatten(self.avgpool(_pair(x)[0]), 1))
         nbt = bn.num_batches_tracked if (bn.training and bn.track_running_stats) else None
         x = bn_relu_maxpool(self.conv1(x), bn.weight, bn.bias, bn.running_mean, bn.running_var,   # fused stem tail
                             training=bn.training or not bn.track_running_stats, momentum=0.1 if bn.momentum is None else bn.momentum,
-                            eps=bn.eps, fused=bn.fused, num_batches_tracked=nbt)
+                            eps=bn.eps, fused=bn.fused, num_batches_tracked=nbt, sync=bn.sync_context())
         x = self.layer4(self.layer3(self.layer2(self.layer1(x))))
         x = _pair(x)[0]               # the last block has a single consumer: its second alias stays unused (gradient None)
         return self.fc(torch.flatten(self.avgpool(x), 1))

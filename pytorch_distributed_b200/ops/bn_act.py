@@ -7,6 +7,9 @@ oracle in ``tests/test_bn_act.py``.
 
 The per-call fp32 accumulators ([2C] sums for forward, [2C] for backward) come from a per-device workspace that is
 zeroed ONCE per training step (one memset for all ~100 slices of a ResNet-50) instead of one ``zeros()`` per layer.
+
+``sync=`` (an ``ops.sync_bn.SyncContext``) normalises with the statistics of the whole data-parallel batch
+(``torch.nn.SyncBatchNorm`` semantics); each direction then takes ``sync_work_len(C)`` floats of the workspace.
 """
 from __future__ import annotations
 
@@ -14,6 +17,8 @@ from typing import Optional
 
 import torch
 import torch.nn.functional as F
+
+from .sync_bn import work_len
 
 
 def bn_act_reference(x, weight, bias, running_mean, running_var, residual=None, relu=True, training=True, momentum=0.1,
@@ -70,7 +75,10 @@ class _Emu:
     """Pure PyTorch (fp32 math) stand-in for the ``csrc/bn_act.cu`` entry points, same signatures and tensor contracts
     (channels_last activations seen as a row-major [M, C] matrix, 1 mask byte per 8 channels, ``saved`` = mean | invstd).
     It documents what the kernels compute and lets the CPU tests drive the autograd plumbing of :class:`_BnActFn`
-    (``bn_act(..., fused="emulate")``)."""
+    (``bn_act(..., fused="emulate")``).  With ``sync`` (a ``SyncContext``) the sums and the row count are added over
+    the ranks with the communicator's ``all_reduce_``."""
+
+    is_emulation = True
 
     @staticmethod
     def _rows(t):
@@ -87,12 +95,26 @@ class _Emu:
         return bits.reshape(m, c).bool()
 
     @staticmethod
-    def bn_act_forward(x, residual, weight, bias, rm, rv, nbt, training, momentum, eps, relu, need_mask, work, stats_ready):
+    def _global_sums(sums, m, sync):
+        """(global [2C] sums, global row count) of this rank's sums over the ranks of ``sync``."""
+        v = torch.cat([sums.float(), sums.new_tensor([float(m)], dtype=torch.float32)])
+        sync.all_reduce_sum_(v)
+        c2 = sums.numel()
+        return v[:c2], int(round(v[c2].item()))
+
+    @staticmethod
+    def bn_act_forward(x, residual, weight, bias, rm, rv, nbt, training, momentum, eps, relu, need_mask, work, stats_ready, sync=None):
         xr = _Emu._rows(x).float()
         m, c = xr.shape
+        n = m                                 # rows the statistics cover
         saved = mask = None
         if training:
-            if stats_ready:
+            if sync is not None:              # E[x^2] - E[x]^2 over the global sums, as the kernels compute it
+                local = work[:2 * c] if stats_ready else torch.cat([xr.sum(0), (xr * xr).sum(0)])
+                g, n = _Emu._global_sums(local, m, sync)
+                mean = g[:c] / n
+                var = (g[c:] / n - mean * mean).clamp_min(0)
+            elif stats_ready:
                 mean = work[:c] / m
                 var = (work[c:2 * c] / m - mean * mean).clamp_min(0)
             else:
@@ -101,7 +123,7 @@ class _Emu:
             saved = torch.cat([mean, invstd])
             if rm is not None:
                 rm.mul_(1 - momentum).add_(momentum * mean)
-                rv.mul_(1 - momentum).add_(momentum * var * (m / (m - 1) if m > 1 else 1.0))
+                rv.mul_(1 - momentum).add_(momentum * var * (n / (n - 1) if n > 1 else 1.0))
             if nbt is not None:
                 nbt.add_(1)
         else:
@@ -117,32 +139,36 @@ class _Emu:
         return _Emu._like(v, x), saved, mask
 
     @staticmethod
-    def _bwd_from_g(g, x, weight, saved):
+    def _bwd_from_g(g, x, weight, saved, sync=None):
         xr = _Emu._rows(x).float()
         m, c = xr.shape
         mean, invstd = saved[:c], saved[c:]
         xhat = (xr - mean) * invstd
         sdz, sdzx = g.sum(0), (g * xhat).sum(0)
-        dx = (weight.float() * invstd) * (g - sdz / m - xhat * sdzx / m)
+        gdz, gdzx, n = sdz, sdzx, m
+        if sync is not None:              # dx from the global sums; dgamma / dbeta stay this rank's
+            tot, n = _Emu._global_sums(torch.cat([sdz, sdzx]), m, sync)
+            gdz, gdzx = tot[:c], tot[c:]
+        dx = (weight.float() * invstd) * (g - gdz / n - xhat * gdzx / n)
         return _Emu._like(dx, x), sdzx.to(weight.dtype), sdz.to(weight.dtype)
 
     @staticmethod
-    def bn_act_backward(dy, x, mask, weight, saved, relu, has_res, work):
+    def bn_act_backward(dy, x, mask, weight, saved, relu, has_res, work, sync=None):
         g = _Emu._rows(dy).float()
         if relu:
             g = g * _Emu._unpack(mask, *g.shape)
-        dx, dw, db = _Emu._bwd_from_g(g, x, weight, saved)
+        dx, dw, db = _Emu._bwd_from_g(g, x, weight, saved, sync)
         dres = None
         if has_res:
             dres = dy if not relu else _Emu._like(g, x)
         return dx, dres, dw, db
 
     @staticmethod
-    def bn_act_backward2(dy_a, dy_b, x, mask, weight, saved, relu, work):
+    def bn_act_backward2(dy_a, dy_b, x, mask, weight, saved, relu, work, sync=None):
         g = (_Emu._rows(dy_a).float() + _Emu._rows(dy_b).float()).to(x.dtype).float()      # rounded like an eager add
         if relu:
             g = g * _Emu._unpack(mask, *g.shape)
-        dx, dw, db = _Emu._bwd_from_g(g, x, weight, saved)
+        dx, dw, db = _Emu._bwd_from_g(g, x, weight, saved, sync)
         return dx, _Emu._like(g, x), dw, db
 
 
@@ -156,25 +182,28 @@ def _kernels(x):
 class _BnActFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x, residual, weight, bias, running_mean, running_var, nbt, training, momentum, eps, relu, need_grad, pre=None,
-                split=False):
+                split=False, sync=None):
         from .. import _ext
         C = _kernels(x)
         ctx.set_materialize_grads(False)
         nc = x.size(1)
         ws = workspace(x.device)
-        stats_ready = pre is not None          # (work[4C], generation): sums already reduced by the producing GEMM
+        wl = work_len(nc, sync)
+        stats_ready = pre is not None          # (work[2 wl], generation): sums already reduced by the producing GEMM
         if stats_ready:
             work, gen = pre
         elif training:
-            work, gen = ws.take(4 * nc)
+            work, gen = ws.take(2 * wl)
         else:
             work, gen = torch.empty(0, dtype=torch.float32, device=x.device), -1
-        _ext.note_launch(1 if (stats_ready or not training) else 3)   # stats + combine + apply
+        _ext.note_launch(1 if (stats_ready or not training) else 3)   # stats + combine (or exchange) + apply
         y, saved, mask = C.bn_act_forward(x, residual, weight, bias, running_mean, running_var, nbt, training, momentum, eps, relu,
-                                          need_grad, work[: 2 * nc] if training else work, stats_ready)
+                                          need_grad, work[:wl] if training else work, stats_ready,
+                                          None if sync is None else sync.kernel_arg(C))
         ctx.relu = relu
         ctx.has_res = residual is not None
-        ctx.work = work[2 * nc:] if training else None
+        ctx.sync = sync
+        ctx.work = work[wl:] if training else None
         ctx.gen = gen
         ctx.ws = ws
         if need_grad:
@@ -188,7 +217,7 @@ class _BnActFn(torch.autograd.Function):
     @staticmethod
     def backward(ctx, dy, dy2=None):
         from .. import _ext
-        none = (None,) * 10
+        none = (None,) * 11
         if dy is None:
             dy, dy2 = dy2, None
         if dy is None:                          # neither alias was used
@@ -196,13 +225,15 @@ class _BnActFn(torch.autograd.Function):
         x, mask, weight, saved = ctx.saved_tensors
         C = _kernels(x)
         work = ctx.work
+        sync = ctx.sync
         if work is None or (ctx.gen != -1 and ctx.gen != ctx.ws.generation):
-            work = torch.zeros(2 * x.size(1), dtype=torch.float32, device=x.device)   # slice was recycled: use a fresh one
-        _ext.note_launch(3)                     # reduce + combine + apply
+            work = torch.zeros(work_len(x.size(1), sync), dtype=torch.float32, device=x.device)   # slice was recycled: use a fresh one
+        _ext.note_launch(3)                     # reduce + combine (or exchange) + apply
+        karg = None if sync is None else sync.kernel_arg(C)
         if dy2 is not None:                     # add + mask + reductions in one pass; g doubles as the residual gradient
-            dx, dres, dw, db = C.bn_act_backward2(dy, dy2, x, mask, weight, saved, ctx.relu, work)
+            dx, dres, dw, db = C.bn_act_backward2(dy, dy2, x, mask, weight, saved, ctx.relu, work, karg)
         else:
-            dx, dres, dw, db = C.bn_act_backward(dy, x, mask, weight, saved, ctx.relu, ctx.has_res, work)
+            dx, dres, dw, db = C.bn_act_backward(dy, x, mask, weight, saved, ctx.relu, ctx.has_res, work, karg)
         return (dx, (dres if ctx.has_res else None), dw, db) + none
 
 
@@ -216,20 +247,81 @@ def _can_fuse(x, weight, residual, running_mean=True, emulate=False) -> bool:
 
 def bn_act(x, weight, bias, running_mean, running_var, residual: Optional[torch.Tensor] = None, relu: bool = True,
            training: bool = True, momentum: float = 0.1, eps: float = 1e-5, fused=None,
-           num_batches_tracked: Optional[torch.Tensor] = None, split: bool = False):
+           num_batches_tracked: Optional[torch.Tensor] = None, split: bool = False, sync=None):
     """relu(batch_norm(x) + residual).  ``fused=None`` picks the CUDA kernels whenever the layout allows it;
     ``fused="emulate"`` runs the same autograd op over the PyTorch emulation of the kernels (CPU tests).
     ``split=True`` returns the result twice - two aliases of one buffer for the two consumers of a residual block's
-    output - so that backward receives their gradients separately and fuses the add (``bn_act_backward2``)."""
-    y = _bn_act(x, weight, bias, running_mean, running_var, residual, relu, training, momentum, eps, fused, num_batches_tracked, split)
+    output - so that backward receives their gradients separately and fuses the add (``bn_act_backward2``).
+    ``sync``: a ``SyncContext`` of world > 1 synchronises the training-mode statistics over the ranks."""
+    if sync is not None and (not training or sync.world == 1):
+        sync = None
+    y = _bn_act(x, weight, bias, running_mean, running_var, residual, relu, training, momentum, eps, fused, num_batches_tracked, split,
+                sync)
     if split and not isinstance(y, tuple):
         return y, y
     return y
 
 
-def _bn_act(x, weight, bias, running_mean, running_var, residual, relu, training, momentum, eps, fused, num_batches_tracked, split):
+class _SyncBnCpuFn(torch.autograd.Function):
+    """Synchronised BatchNorm in plain PyTorch over the communicator's ``all_reduce_`` (torch's SyncBatchNorm function has
+    no CPU kernels): the same statistics contract as the fused kernels, any layout."""
+
+    @staticmethod
+    def forward(ctx, x, weight, bias, running_mean, running_var, eps, momentum, sync):
+        c = x.size(1)
+        xf = x.float()
+        dims = [d for d in range(x.dim()) if d != 1]
+        shape = [1, c] + [1] * (x.dim() - 2)
+        g, n = _Emu._global_sums(torch.cat([xf.sum(dims), (xf * xf).sum(dims)]), x.numel() // c, sync)
+        mean = g[:c] / n
+        var = (g[c:] / n - mean * mean).clamp_min(0)
+        invstd = torch.rsqrt(var + eps)
+        if running_mean is not None:
+            running_mean.mul_(1 - momentum).add_(momentum * mean)
+            running_var.mul_(1 - momentum).add_(momentum * var * (n / (n - 1) if n > 1 else 1.0))
+        xhat = (xf - mean.view(shape)) * invstd.view(shape)
+        ctx.save_for_backward(xhat, weight, invstd)
+        ctx.sync, ctx.dims, ctx.shape = sync, dims, shape
+        return (xhat * weight.float().view(shape) + bias.float().view(shape)).to(x.dtype)
+
+    @staticmethod
+    def backward(ctx, dy):
+        xhat, weight, invstd = ctx.saved_tensors
+        c, shape = xhat.size(1), ctx.shape
+        g = dy.float()
+        sdz, sdzx = g.sum(ctx.dims), (g * xhat).sum(ctx.dims)
+        tot, n = _Emu._global_sums(torch.cat([sdz, sdzx]), xhat.numel() // c, ctx.sync)
+        dx = (weight.float() * invstd).view(shape) * (g - (tot[:c] / n).view(shape) - xhat * (tot[c:] / n).view(shape))
+        return dx.to(dy.dtype), sdzx.to(weight.dtype), sdz.to(weight.dtype), None, None, None, None, None
+
+
+def sync_batch_norm_unfused(x, weight, bias, running_mean, running_var, momentum, eps, num_batches_tracked, sync):
+    """Layers the fused kernels cannot take (NCHW, C % 8 != 0, ...) and communicators other than the fused one: on CUDA
+    ``torch.nn.SyncBatchNorm``'s own autograd function over the communicator's process group, on CPU the same semantics
+    over the communicator's ``all_reduce_``."""
+    if num_batches_tracked is not None:
+        num_batches_tracked.add_(1)
+    if not x.is_cuda:
+        return _SyncBnCpuFn.apply(x, weight, bias, running_mean, running_var, eps, momentum, sync)
+    if torch.cuda.is_current_stream_capturing():
+        raise RuntimeError("synchronised BatchNorm on a layer the fused kernels cannot take (NCHW, C % 8 != 0, --no-fused-bn) "
+                           "runs torch.distributed collectives, which a CUDA graph cannot capture")
+    from torch.nn.modules._functions import SyncBatchNorm as _TorchSyncBN
+    if weight is not None and weight.dtype != x.dtype:
+        weight, bias = weight.to(x.dtype), bias.to(x.dtype)
+    group = getattr(sync.comm, "group", None) or torch.distributed.group.WORLD
+    return _TorchSyncBN.apply(x, weight, bias, running_mean, running_var, eps, momentum, group, sync.world)
+
+
+def _bn_act(x, weight, bias, running_mean, running_var, residual, relu, training, momentum, eps, fused, num_batches_tracked, split,
+            sync=None):
     ok = _can_fuse(x, weight, residual, running_mean, emulate=(fused == "emulate"))
     use = ok if fused is None else (bool(fused) and ok)
+    if sync is not None and (not use or (x.is_cuda and sync.native is None)):
+        y = sync_batch_norm_unfused(x, weight, bias, running_mean, running_var, momentum, eps, num_batches_tracked, sync)
+        if residual is not None:
+            y = y + residual
+        return F.relu(y) if relu else y
     if not use:
         if weight is not None and x.is_cuda and weight.dtype != torch.float32 and x.dtype != weight.dtype:
             weight, bias = weight.to(x.dtype), bias.to(x.dtype)
@@ -249,4 +341,4 @@ def _bn_act(x, weight, bias, running_mean, running_var, residual, relu, training
                                 bias.to(x.dtype) if bias.dtype != torch.float32 else bias, running_mean, running_var, residual, relu,
                                 training, momentum, eps)
     return _BnActFn.apply(x, residual, weight, bias, running_mean, running_var, num_batches_tracked, training, float(momentum),
-                          float(eps), relu, need_grad, None, bool(split and need_grad))
+                          float(eps), relu, need_grad, None, bool(split and need_grad), sync)

@@ -15,14 +15,15 @@ from __future__ import annotations
 import torch
 
 from .bn_act import _BnActFn, _can_fuse, workspace
+from .sync_bn import work_len
 
 
 class _Conv1x1Stats(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, x, weight, stats):
+    def forward(ctx, x, weight, stats, sync=None):
         from .. import _ext
-        _ext.note_launch(2)                     # GEMM + statistics combine
-        y = _ext.lib().conv1x1_bnstats(x, weight, stats)
+        _ext.note_launch(2)                     # GEMM + statistics combine (or cross-rank exchange)
+        y = _ext.lib().conv1x1_bnstats(x, weight, stats, sync)
         ctx.save_for_backward(x, weight)
         return y
 
@@ -32,7 +33,7 @@ class _Conv1x1Stats(torch.autograd.Function):
         dy = dy.contiguous(memory_format=torch.channels_last)
         dx, dw, _ = torch.ops.aten.convolution_backward(dy, x, weight, None, (1, 1), (0, 0), (1, 1), False, (0, 0), 1,
                                                         (ctx.needs_input_grad[0], ctx.needs_input_grad[1], False))
-        return dx, dw, None
+        return dx, dw, None, None
 
 
 GEMM_DTYPES = (torch.bfloat16, torch.float16)
@@ -62,21 +63,24 @@ def can_fuse_conv1x1(x, conv) -> bool:
 
 
 def conv1x1_bn_act(x, conv, bn, residual=None, enabled=True, split=False):
-    """relu?(bn(conv1x1(x)) + residual) for a ``nn.Conv2d`` and a :class:`BNAct` module (``split``: see ``bn_act``)."""
+    """relu?(bn(conv1x1(x)) + residual) for a ``nn.Conv2d`` and a :class:`BNAct` module (``split``: see ``bn_act``).
+    A synchronised ``bn`` (``SyncBNAct``) exchanges the GEMM's statistics across the ranks before the apply pass."""
     training = bn.training or not bn.track_running_stats
-    if not (enabled and training and can_fuse_conv1x1(x, conv) and bn.fused is not False):
+    sync = bn.sync_context()
+    if not (enabled and training and can_fuse_conv1x1(x, conv) and bn.fused is not False and (sync is None or sync.native is not None)):
         return bn(conv(x), residual, split) if split else bn(conv(x), residual)
     nc = conv.weight.size(0)
     ws = workspace(x.device)
-    work, gen = ws.take(4 * nc)
-    y = _Conv1x1Stats.apply(x, gemm_weight(conv.weight, autocast_gemm_dtype()), work[: 2 * nc])
+    wl = work_len(nc, sync)
+    work, gen = ws.take(2 * wl)
+    y = _Conv1x1Stats.apply(x, gemm_weight(conv.weight, autocast_gemm_dtype()), work[:wl], None if sync is None else sync.native)
     if not _can_fuse(y, bn.weight, residual, bn.running_mean):
         return bn(y, residual, split) if split else bn(y, residual)   # (cannot happen for the shapes accepted above)
     need_grad = torch.is_grad_enabled() and (y.requires_grad or bn.weight.requires_grad)
     nbt = bn.num_batches_tracked if (bn.training and bn.track_running_stats) else None
     out = _BnActFn.apply(y, residual, bn.weight, bn.bias, bn.running_mean, bn.running_var, nbt, True,
                          0.1 if bn.momentum is None else float(bn.momentum), float(bn.eps), bn.relu, need_grad, (work, gen),
-                         bool(split and need_grad))
+                         bool(split and need_grad), sync)
     if split and not isinstance(out, tuple):
         return out, out
     return out

@@ -8,7 +8,8 @@ from __future__ import annotations
 import torch
 import torch.nn.functional as F
 
-from .bn_act import bn_act_reference, workspace
+from .bn_act import bn_act_reference, sync_batch_norm_unfused, workspace
+from .sync_bn import work_len
 
 
 def bn_relu_maxpool_reference(x, weight, bias, running_mean, running_var, training=True, momentum=0.1, eps=1e-5):
@@ -18,20 +19,21 @@ def bn_relu_maxpool_reference(x, weight, bias, running_mean, running_var, traini
 
 class _StemFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, x, weight, bias, running_mean, running_var, nbt, training, momentum, eps, need_grad):
+    def forward(ctx, x, weight, bias, running_mean, running_var, nbt, training, momentum, eps, need_grad, sync=None):
         from .. import _ext
         C = _ext.lib()
         nc = x.size(1)
         ws = workspace(x.device)
+        wl = work_len(nc, sync)
         if training:
-            work, gen = ws.take(4 * nc)
+            work, gen = ws.take(2 * wl)
         else:
             work, gen = torch.empty(0, dtype=torch.float32, device=x.device), -1
         _ext.note_launch(3 if training else 1)
         y, saved, code = C.stem_forward(x, weight, bias, running_mean, running_var, nbt, training, momentum, eps, need_grad,
-                                        work[: 2 * nc] if training else work)
-        ctx.work = work[2 * nc:] if training else None
-        ctx.gen, ctx.ws = gen, ws
+                                        work[:wl] if training else work, None if sync is None else sync.native)
+        ctx.work = work[wl:] if training else None
+        ctx.gen, ctx.ws, ctx.sync = gen, ws, sync
         if need_grad:
             if not training:
                 raise RuntimeError("fused stem: backward through eval-mode batch norm is not supported")
@@ -44,11 +46,12 @@ class _StemFn(torch.autograd.Function):
         C = _ext.lib()
         x, code, weight, saved = ctx.saved_tensors
         work = ctx.work
+        sync = ctx.sync
         if work is None or (ctx.gen != -1 and ctx.gen != ctx.ws.generation):
-            work = torch.zeros(2 * x.size(1), dtype=torch.float32, device=x.device)
+            work = torch.zeros(work_len(x.size(1), sync), dtype=torch.float32, device=x.device)
         _ext.note_launch(3)
-        dx, dw, db = C.stem_backward(dy, x, code, weight, saved, work)
-        return dx, dw, db, None, None, None, None, None, None, None
+        dx, dw, db = C.stem_backward(dy, x, code, weight, saved, work, None if sync is None else sync.native)
+        return dx, dw, db, None, None, None, None, None, None, None, None
 
 
 def can_fuse_stem(x, weight, running_mean) -> bool:
@@ -59,12 +62,19 @@ def can_fuse_stem(x, weight, running_mean) -> bool:
 
 
 def bn_relu_maxpool(x, weight, bias, running_mean, running_var, training=True, momentum=0.1, eps=1e-5, fused=None,
-                    num_batches_tracked=None):
+                    num_batches_tracked=None, sync=None):
+    """maxpool(relu(bn(x))); ``sync`` (a ``SyncContext``, see ``ops/sync_bn.py``) synchronises the training statistics."""
+    if sync is not None and (not training or sync.world == 1):
+        sync = None
     ok = can_fuse_stem(x, weight, running_mean)
     need_grad = torch.is_grad_enabled() and (x.requires_grad or (weight is not None and weight.requires_grad))
     if need_grad and not training:
         ok = False
-    if not (ok if fused is None else (fused and ok)):
+    use = ok if fused is None else (fused and ok)
+    if sync is not None and not (use and sync.native is not None):
+        y = sync_batch_norm_unfused(x, weight, bias, running_mean, running_var, momentum, eps, num_batches_tracked, sync)
+        return F.max_pool2d(F.relu(y), kernel_size=3, stride=2, padding=1)
+    if not use:
         if training and num_batches_tracked is not None:
             num_batches_tracked.add_(1)
         if weight is not None and x.is_cuda and weight.dtype != torch.float32 and x.dtype != weight.dtype:
@@ -73,4 +83,5 @@ def bn_relu_maxpool(x, weight, bias, running_mean, running_var, training=True, m
             return bn_relu_maxpool_reference(x.float(), weight.float(), bias.float(), running_mean, running_var, training, momentum,
                                              eps).to(x.dtype)
         return bn_relu_maxpool_reference(x, weight, bias, running_mean, running_var, training, momentum, eps)
-    return _StemFn.apply(x, weight, bias, running_mean, running_var, num_batches_tracked, training, float(momentum), float(eps), need_grad)
+    return _StemFn.apply(x, weight, bias, running_mean, running_var, num_batches_tracked, training, float(momentum), float(eps), need_grad,
+                         sync)

@@ -21,6 +21,7 @@ import torch
 import torch.nn.functional as F
 
 from .bn_act import workspace
+from .sync_bn import work_len
 from .conv_bn import GEMM_DTYPES, autocast_gemm_dtype, gemm_weight
 from .stem import _StemFn, bn_relu_maxpool, can_fuse_stem
 
@@ -71,7 +72,7 @@ class _StemConvFn(torch.autograd.Function):
     """y = conv7x7s2(x, weight) through im2col + GEMM; ``stats`` (zeroed fp32 [2 * C_out]) receives sum / sum of squares."""
 
     @staticmethod
-    def forward(ctx, x, weight, stats, emulate=False):
+    def forward(ctx, x, weight, stats, emulate=False, sync=None):
         packed = pack_stem_weight(weight)
         if emulate:
             a = im2col_reference(x).contiguous(memory_format=torch.channels_last)
@@ -86,7 +87,7 @@ class _StemConvFn(torch.autograd.Function):
             C = _ext.lib()
             _ext.note_launch(3)                 # im2col + GEMM + statistics combine
             a = C.stem_im2col(x)
-            y = C.conv1x1_bnstats(a, packed.view(packed.size(0), K_PAD, 1, 1), stats)
+            y = C.conv1x1_bnstats(a, packed.view(packed.size(0), K_PAD, 1, 1), stats, sync)
         ctx.save_for_backward(a, weight)
         return y
 
@@ -104,21 +105,21 @@ class _StemConvFn(torch.autograd.Function):
             dwp = torch.mm(dy2.t(), rows, out_dtype=torch.float32)
         else:
             dwp = dy2.float().t() @ rows.float()
-        return None, unpack_stem_weight(dwp, weight), None, None
+        return None, unpack_stem_weight(dwp, weight), None, None, None
 
 
 class _StemPreFn(torch.autograd.Function):
     """The fused stem tail (BN + ReLU + MaxPool) when the producing GEMM has already reduced the BN statistics."""
 
     @staticmethod
-    def forward(ctx, x, weight, bias, running_mean, running_var, nbt, momentum, eps, need_grad, work, gen):
+    def forward(ctx, x, weight, bias, running_mean, running_var, nbt, momentum, eps, need_grad, work, gen, sync=None):
         from .. import _ext
-        nc = x.size(1)
+        wl = work_len(x.size(1), sync)
         _ext.note_launch(1)
         y, saved, code = _ext.lib().stem_forward_pre(x, weight, bias, running_mean, running_var, nbt, True, momentum, eps, need_grad,
-                                                     work[: 2 * nc])
-        ctx.work = work[2 * nc:]
-        ctx.gen, ctx.ws = gen, workspace(x.device)
+                                                     work[:wl], None if sync is None else sync.native)
+        ctx.work = work[wl:]
+        ctx.gen, ctx.ws, ctx.sync = gen, workspace(x.device), sync
         if need_grad:
             ctx.save_for_backward(x, code, weight, saved)
         return y
@@ -129,21 +130,26 @@ class _StemPreFn(torch.autograd.Function):
 
 
 def stem_conv_bn_relu_maxpool(x, conv, bn, emulate: bool = False):
-    """maxpool(relu(bn(conv7x7(x)))) for the ResNet stem modules ``conv`` (nn.Conv2d) and ``bn`` (BNAct), training mode."""
+    """maxpool(relu(bn(conv7x7(x)))) for the ResNet stem modules ``conv`` (nn.Conv2d) and ``bn`` (BNAct), training mode.
+    A synchronised ``bn`` (``SyncBNAct``) exchanges the GEMM's statistics across the ranks."""
     nc = conv.weight.size(0)
     momentum = 0.1 if bn.momentum is None else float(bn.momentum)
     nbt = bn.num_batches_tracked if (bn.training and bn.track_running_stats) else None
+    sync = bn.sync_context()
     if emulate:                                                        # CPU / test path: same op graph, PyTorch math
         y = _StemConvFn.apply(x, conv.weight, None, True)
         return bn_relu_maxpool(y, bn.weight, bn.bias, bn.running_mean, bn.running_var, training=True, momentum=momentum, eps=bn.eps,
-                               fused=False, num_batches_tracked=nbt)
+                               fused=False, num_batches_tracked=nbt, sync=sync)
     ac = autocast_gemm_dtype()
     if ac is not None and x.dtype != ac:
         x = x.to(ac)                                                   # keeps channels_last
     ws = workspace(x.device)
-    work, gen = ws.take(4 * nc)
-    y = _StemConvFn.apply(x, gemm_weight(conv.weight, ac), work[: 2 * nc], False)   # always 4 inputs: backward returns 4 gradients
+    wl = work_len(nc, sync)
+    work, gen = ws.take(2 * wl)
+    native = None if sync is None else sync.native
+    y = _StemConvFn.apply(x, gemm_weight(conv.weight, ac), work[:wl], False, native)   # always 5 inputs: backward returns 5 gradients
     if not can_fuse_stem(y, bn.weight, bn.running_mean):
         raise RuntimeError("stem GEMM output does not fit the fused stem tail")
     need_grad = torch.is_grad_enabled() and (y.requires_grad or bn.weight.requires_grad)
-    return _StemPreFn.apply(y, bn.weight, bn.bias, bn.running_mean, bn.running_var, nbt, momentum, float(bn.eps), need_grad, work, gen)
+    return _StemPreFn.apply(y, bn.weight, bn.bias, bn.running_mean, bn.running_var, nbt, momentum, float(bn.eps), need_grad, work, gen,
+                            sync)

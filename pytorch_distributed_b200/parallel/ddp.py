@@ -402,6 +402,8 @@ class DistributedDataParallel(nn.Module):
         if isinstance(comm, str):
             comm = make_communicator(comm, group=process_group, device=self.device)
         self.comm = comm
+        from ..utils.dist_ops import register_for_sync_batchnorm
+        register_for_sync_batchnorm(module, comm)
         if wire_dtype is None:
             if gradient_as_bucket_view and self.device.type == "cuda":
                 wire_dtype = _WIRE_OF.get(params[0].dtype, "bf16")       # bucket views carry the gradients' own dtype

@@ -81,6 +81,13 @@ def communicator():
     return _state["comm"]
 
 
+def __getattr__(name):
+    if name == "SyncBatchNorm":       # hvd.SyncBatchNorm (lazy: the models import this package's ops)
+        from ..models.resnet import SyncBNAct
+        return SyncBNAct
+    raise AttributeError(name)
+
+
 def nccl_built() -> bool:
     return False      # the data plane is hand-written peer-memory kernels, not NCCL
 

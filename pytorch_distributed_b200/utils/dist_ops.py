@@ -21,6 +21,22 @@ def set_default_communicator(comm) -> None:
     _default_comm = comm
 
 
+def default_communicator():
+    """The communicator synchronised BatchNorm layers bind to: the one registered for this process (this package's DDP
+    and apex DDP register theirs when the model has synchronised layers), else ``hvd.init()``'s, else None."""
+    if _default_comm is not None:
+        return _default_comm
+    from ..parallel import hvd
+    return hvd.communicator() if hvd.is_initialized() else None
+
+
+def register_for_sync_batchnorm(module, comm) -> None:
+    """Register ``comm`` for the synchronised BatchNorm layers of ``module`` (if it has any and none is registered yet)."""
+    from ..models.resnet import SyncBNAct
+    if _default_comm is None and any(isinstance(m, SyncBNAct) for m in module.modules()):
+        set_default_communicator(comm)
+
+
 def reduce_mean(tensor: torch.Tensor, nprocs: Optional[int] = None, comm=None) -> torch.Tensor:
     rt = tensor.detach().clone()
     comm = comm or _default_comm
