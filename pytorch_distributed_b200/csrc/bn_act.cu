@@ -10,8 +10,8 @@
 // Layout: activations are channels_last, i.e. a row-major [M = N*H*W, C] matrix.  A thread owns 8 consecutive
 // channels (one 16-byte vector for 16-bit dtypes) and walks down the rows, so every warp access is a fully
 // coalesced 128..512-byte line and the per-channel reductions stay in registers until the end of the CTA.
-// CTA-level combine: warp shuffles (lanes sharing a channel group) -> one shared-memory row per warp/row-group
-// (plain stores, no shared atomics) -> one fire-and-forget global fp32 RED per (CTA, channel).
+// CTA-level combine (cta_combine): warp shuffles (lanes sharing a channel group) -> one shared-memory row per warp/row-group
+// (plain stores, no shared atomics) -> one row of partial sums per CTA; finish_sums() adds the rows in a fixed order.
 #include <ATen/cuda/CUDAContext.h>
 #include <c10/cuda/CUDAGuard.h>
 #include <torch/extension.h>
@@ -469,54 +469,57 @@ static int apply_grid(const Geometry& g) {
   return (int)std::max<int64_t>(std::min<int64_t>(blocks, (int64_t)g.sms * 8), 1);
 }
 
+template <typename T> struct Tag { using type = T; };
+// f(Tag<T>{}) with T the element type of the activations x
+template <typename F>
+static void for_act_dtype(const at::Tensor& x, F&& f) {
+  switch (x.scalar_type()) {
+    case at::kBFloat16: f(Tag<__nv_bfloat16>{}); break;
+    case at::kHalf: f(Tag<__half>{}); break;
+    case at::kFloat: f(Tag<float>{}); break;
+    default: TORCH_CHECK(false, "unsupported activation dtype");
+  }
+}
+
+template <typename U>
+static U* ptr_or_null(const at::Tensor& t) { return t.defined() ? t.data_ptr<U>() : nullptr; }
+
+// The per-channel sum / sum of squares a forward apply kernel reads from `work`.  reduce: one statistics pass over x adds
+// them there first; otherwise they are in place already (eval mode reads none; stats_ready: the producing GEMM reduced
+// them, gemm_bnstats.cu).
+template <typename T>
+static const float* forward_sums(const at::Tensor& x, const Geometry& g, const at::Tensor& work, bool reduce, const SyncBN* sync,
+                                 cudaStream_t st) {
+  float* wk = ptr_or_null<float>(work);
+  if (!reduce) return work_sums(wk, g.C, sync);
+  int rpb;
+  const int grid = reduce_grid(g, &rpb, resident_ctas(bn_stats_kernel<T>, g.smem));
+  at::Tensor part = partials(x, grid, g.C);
+  bn_stats_kernel<T><<<grid, kBnThreads, g.smem, st>>>(reinterpret_cast<const T*>(x.data_ptr()), part.data_ptr<float>(), g.M, g.C, rpb);
+  C10_CUDA_KERNEL_LAUNCH_CHECK();
+  return finish_sums(part.data_ptr<float>(), grid, g.C, g.M, wk, sync, st);
+}
+
 template <typename T>
 static void fwd_impl(const at::Tensor& x, const at::Tensor* res, at::Tensor& y, at::Tensor& mask, at::Tensor& work, at::Tensor& saved,
                      const at::Tensor& w, const at::Tensor& b, at::Tensor& rm, at::Tensor& rv, at::Tensor& nbt, bool training, float momentum,
                      float eps, bool relu, bool stats_ready, const SyncBN* sync) {
   const Geometry g = geometry(x);
   cudaStream_t st = at::cuda::getCurrentCUDAStream();
-  const T* xp = reinterpret_cast<const T*>(x.data_ptr());
-  T* yp = reinterpret_cast<T*>(y.data_ptr());
-  const T* rp = res ? reinterpret_cast<const T*>(res->data_ptr()) : nullptr;
-  float* wk = work.defined() ? work.data_ptr<float>() : nullptr;
-  if (training && !stats_ready) {     // stats_ready: the producing GEMM already reduced sum / sum-of-squares (gemm_bnstats.cu)
-    int rpb;
-    const int grid = reduce_grid(g, &rpb, resident_ctas(bn_stats_kernel<T>, g.smem));
-    at::Tensor part = partials(x, grid, g.C);
-    bn_stats_kernel<T><<<grid, kBnThreads, g.smem, st>>>(xp, part.data_ptr<float>(), g.M, g.C, rpb);
-    C10_CUDA_KERNEL_LAUNCH_CHECK();
-    if (sync) sync_bn_exchange(part.data_ptr<float>(), grid, g.C, g.M, wk, *sync, st);
-    else combine_partials(part.data_ptr<float>(), grid, 2 * g.C, wk, st);
-  }
-  const int grid = apply_grid(g);
-  float* rmp = rm.defined() ? rm.data_ptr<float>() : nullptr;
-  float* rvp = rv.defined() ? rv.data_ptr<float>() : nullptr;
-  int64_t* nb = nbt.defined() ? nbt.data_ptr<int64_t>() : nullptr;
-  float* sv = saved.defined() ? saved.data_ptr<float>() : nullptr;
-  uint8_t* mk = mask.defined() ? mask.data_ptr<uint8_t>() : nullptr;
-  const int wdt = wdtype(w);
-#define APPLY(K, R, S) \
-  K<T, R, S><<<grid, kBnThreads, 0, st>>>(xp, rp, yp, mk, wk, w.data_ptr(), b.data_ptr(), wdt, rmp, rvp, nb, sv, g.M, g.C, eps, momentum, training ? 1 : 0)
-  if (sync) {                         // the apply reads the global sums and count
-    wk += 2 * g.C;
-    if (relu) { if (res) APPLY(bn_apply_sync_kernel, true, true); else APPLY(bn_apply_sync_kernel, true, false); }
-    else      { if (res) APPLY(bn_apply_sync_kernel, false, true); else APPLY(bn_apply_sync_kernel, false, false); }
-  } else {
-    if (relu) { if (res) APPLY(bn_apply_kernel, true, true); else APPLY(bn_apply_kernel, true, false); }
-    else      { if (res) APPLY(bn_apply_kernel, false, true); else APPLY(bn_apply_kernel, false, false); }
-  }
-#undef APPLY
+  const float* sums = forward_sums<T>(x, g, work, training && !stats_ready, sync, st);
+  using K = decltype(&bn_apply_kernel<T, false, false>);
+  static constexpr K kernels[2][2][2] = {             // [sync][relu][res]
+      {{bn_apply_kernel<T, false, false>, bn_apply_kernel<T, false, true>}, {bn_apply_kernel<T, true, false>, bn_apply_kernel<T, true, true>}},
+      {{bn_apply_sync_kernel<T, false, false>, bn_apply_sync_kernel<T, false, true>},
+       {bn_apply_sync_kernel<T, true, false>, bn_apply_sync_kernel<T, true, true>}}};
+  kernels[sync != nullptr][relu][res != nullptr]<<<apply_grid(g), kBnThreads, 0, st>>>(
+      reinterpret_cast<const T*>(x.data_ptr()), res ? reinterpret_cast<const T*>(res->data_ptr()) : nullptr, reinterpret_cast<T*>(y.data_ptr()),
+      ptr_or_null<uint8_t>(mask), sums, w.data_ptr(), b.data_ptr(), wdtype(w), ptr_or_null<float>(rm), ptr_or_null<float>(rv),
+      ptr_or_null<int64_t>(nbt), ptr_or_null<float>(saved), g.M, g.C, eps, momentum, training ? 1 : 0);
   C10_CUDA_KERNEL_LAUNCH_CHECK();
 }
 
-// A synchronised call needs a training-mode work slice of the exchange layout (host.h: kSyncWork)
-static void check_sync_work(const SyncBN* sync, const at::Tensor& work, int64_t C) {
-  if (!sync) return;
-  TORCH_CHECK(work.defined() && work.scalar_type() == at::kFloat && work.numel() >= kSyncWork(C),
-              "synchronised BatchNorm needs a work slice of ", kSyncWork(C), " floats");
-}
-
-// returns {y, saved(mean|invstd), relu_mask}; `work` = zeroed float[2C] accumulator supplied by the caller
+// returns {y, saved(mean|invstd), relu_mask}; `work` = the zeroed accumulator slice supplied by the caller (host.h: check_work)
 std::vector<at::Tensor> bn_act_forward(const at::Tensor& x, const c10::optional<at::Tensor>& residual, const at::Tensor& weight,
                                        const at::Tensor& bias, at::Tensor running_mean, at::Tensor running_var,
                                        c10::optional<at::Tensor> num_batches_tracked, bool training, double momentum, double eps, bool relu,
@@ -541,18 +544,35 @@ std::vector<at::Tensor> bn_act_forward(const at::Tensor& x, const c10::optional<
     TORCH_CHECK(nbt.scalar_type() == at::kLong && nbt.is_cuda());
   }
   if (training) {
-    TORCH_CHECK(work.defined() && work.scalar_type() == at::kFloat && work.numel() >= 2 * C, "work buffer too small");
+    check_work(work, C, sync);
     saved = at::empty({2 * C}, x.options().dtype(at::kFloat));
   }
-  check_sync_work(sync, work, C);
   if (relu && need_mask) mask = at::empty({x.numel() / 8}, x.options().dtype(at::kByte));
-  switch (x.scalar_type()) {
-    case at::kBFloat16: fwd_impl<__nv_bfloat16>(x, res, y, mask, work, saved, weight, bias, running_mean, running_var, nbt, training, (float)momentum, (float)eps, relu, stats_ready, sync); break;
-    case at::kHalf: fwd_impl<__half>(x, res, y, mask, work, saved, weight, bias, running_mean, running_var, nbt, training, (float)momentum, (float)eps, relu, stats_ready, sync); break;
-    case at::kFloat: fwd_impl<float>(x, res, y, mask, work, saved, weight, bias, running_mean, running_var, nbt, training, (float)momentum, (float)eps, relu, stats_ready, sync); break;
-    default: TORCH_CHECK(false, "unsupported activation dtype");
-  }
+  for_act_dtype(x, [&](auto t) {
+    fwd_impl<typename decltype(t)::type>(x, res, y, mask, work, saved, weight, bias, running_mean, running_var, nbt, training, (float)momentum,
+                                         (float)eps, relu, stats_ready, sync);
+  });
   return {y, saved, mask};
+}
+
+// Second pass of a BatchNorm backward: finish the reduction pass's partials, then dx (and dres = dz with `dres`) from
+// dz = dy (x the ReLU mask bits with `relu`).
+template <typename T>
+static void bwd_apply(const Geometry& g, const at::Tensor& part, const T* dy, const uint8_t* mask, const at::Tensor& x, const at::Tensor& saved,
+                      at::Tensor& work, const at::Tensor& w, at::Tensor& dx, T* dres, at::Tensor& dw, at::Tensor& db, bool relu,
+                      const SyncBN* sync, cudaStream_t st) {
+  using K = decltype(&bn_bwd_apply_kernel<T, false, false>);
+  static constexpr K kernels[2][2][2] = {             // [sync][relu][res]
+      {{bn_bwd_apply_kernel<T, false, false>, bn_bwd_apply_kernel<T, false, true>},
+       {bn_bwd_apply_kernel<T, true, false>, bn_bwd_apply_kernel<T, true, true>}},
+      {{bn_bwd_apply_sync_kernel<T, false, false>, bn_bwd_apply_sync_kernel<T, false, true>},
+       {bn_bwd_apply_sync_kernel<T, true, false>, bn_bwd_apply_sync_kernel<T, true, true>}}};
+  const int wdt = wdtype(w);
+  const float* sums = finish_sums(part.data_ptr<float>(), (int)part.size(0), g.C, g.M, work.data_ptr<float>(), sync, st);
+  kernels[sync != nullptr][relu][dres != nullptr]<<<apply_grid(g), kBnThreads, 0, st>>>(
+      dy, mask, reinterpret_cast<const T*>(x.data_ptr()), saved.data_ptr<float>(), sums, w.data_ptr(), wdt, reinterpret_cast<T*>(dx.data_ptr()),
+      dres, dw.data_ptr(), db.data_ptr(), g.M, g.C);
+  C10_CUDA_KERNEL_LAUNCH_CHECK();
 }
 
 template <typename T>
@@ -563,35 +583,14 @@ static void bwd_impl(const at::Tensor& dy, const at::Tensor& mask, const at::Ten
   cudaStream_t st = at::cuda::getCurrentCUDAStream();
   const T* dyp = reinterpret_cast<const T*>(dy.data_ptr());
   const uint8_t* mk = relu ? mask.data_ptr<uint8_t>() : nullptr;
-  const T* xp = reinterpret_cast<const T*>(x.data_ptr());
-  float* wk = work.data_ptr<float>();
-  const float* sv = saved.data_ptr<float>();
+  const auto reduce = relu ? bn_bwd_reduce_kernel<T, true> : bn_bwd_reduce_kernel<T, false>;
   int rpb;
-  const int rgrid = reduce_grid(g, &rpb, relu ? resident_ctas(bn_bwd_reduce_kernel<T, true>, g.smem)
-                                             : resident_ctas(bn_bwd_reduce_kernel<T, false>, g.smem));
+  const int rgrid = reduce_grid(g, &rpb, resident_ctas(reduce, g.smem));
   at::Tensor part = partials(x, rgrid, g.C);
-  float* pp = part.data_ptr<float>();
-  if (relu) bn_bwd_reduce_kernel<T, true><<<rgrid, kBnThreads, g.smem, st>>>(dyp, mk, xp, sv, pp, g.M, g.C, rpb);
-  else      bn_bwd_reduce_kernel<T, false><<<rgrid, kBnThreads, g.smem, st>>>(dyp, mk, xp, sv, pp, g.M, g.C, rpb);
+  reduce<<<rgrid, kBnThreads, g.smem, st>>>(dyp, mk, reinterpret_cast<const T*>(x.data_ptr()), saved.data_ptr<float>(), part.data_ptr<float>(),
+                                            g.M, g.C, rpb);
   C10_CUDA_KERNEL_LAUNCH_CHECK();
-  const int grid = apply_grid(g);
-  T* dxp = reinterpret_cast<T*>(dx.data_ptr());
-  T* drp = write_res ? reinterpret_cast<T*>(dres.data_ptr()) : nullptr;
-  const int wdt = wdtype(w);
-#define BAPPLY(K, R, S) \
-  K<T, R, S><<<grid, kBnThreads, 0, st>>>(dyp, mk, xp, sv, wk, w.data_ptr(), wdt, dxp, drp, dw.data_ptr(), db.data_ptr(), g.M, g.C)
-  if (sync) {
-    sync_bn_exchange(pp, rgrid, g.C, g.M, wk, *sync, st);
-    wk += 2 * g.C;
-    if (relu) { if (write_res) BAPPLY(bn_bwd_apply_sync_kernel, true, true); else BAPPLY(bn_bwd_apply_sync_kernel, true, false); }
-    else      { if (write_res) BAPPLY(bn_bwd_apply_sync_kernel, false, true); else BAPPLY(bn_bwd_apply_sync_kernel, false, false); }
-  } else {
-    combine_partials(pp, rgrid, 2 * g.C, wk, st);
-    if (relu) { if (write_res) BAPPLY(bn_bwd_apply_kernel, true, true); else BAPPLY(bn_bwd_apply_kernel, true, false); }
-    else      { if (write_res) BAPPLY(bn_bwd_apply_kernel, false, true); else BAPPLY(bn_bwd_apply_kernel, false, false); }
-  }
-#undef BAPPLY
-  C10_CUDA_KERNEL_LAUNCH_CHECK();
+  bwd_apply<T>(g, part, dyp, mk, x, saved, work, w, dx, write_res ? reinterpret_cast<T*>(dres.data_ptr()) : nullptr, dw, db, relu, sync, st);
 }
 
 // returns {dx, dres (undefined if !has_residual), dweight, dbias}
@@ -607,21 +606,14 @@ std::vector<at::Tensor> bn_act_backward(const at::Tensor& dy_in, const at::Tenso
                 "ReLU backward needs the forward's bit mask");
     mask = *mask_opt;
   }
-  const int C = (int)x.size(1);
-  TORCH_CHECK(work.defined() && work.scalar_type() == at::kFloat && work.numel() >= 2 * C, "work buffer too small");
+  check_work(work, x.size(1), sync);
   c10::cuda::CUDAGuard guard(x.device());
   at::Tensor dx = at::empty_like(x, x.options().memory_format(at::MemoryFormat::ChannelsLast));
   at::Tensor dres;
   if (has_residual) dres = (!relu) ? dy : at::empty_like(x, x.options().memory_format(at::MemoryFormat::ChannelsLast));
   at::Tensor dw = at::empty_like(weight), db = at::empty_like(weight);
   const bool write_res = has_residual && relu;  // without ReLU the residual gradient IS dy: no copy
-  check_sync_work(sync, work, C);
-  switch (x.scalar_type()) {
-    case at::kBFloat16: bwd_impl<__nv_bfloat16>(dy, mask, x, saved, work, weight, dx, dres, dw, db, relu, write_res, sync); break;
-    case at::kHalf: bwd_impl<__half>(dy, mask, x, saved, work, weight, dx, dres, dw, db, relu, write_res, sync); break;
-    case at::kFloat: bwd_impl<float>(dy, mask, x, saved, work, weight, dx, dres, dw, db, relu, write_res, sync); break;
-    default: TORCH_CHECK(false, "unsupported activation dtype");
-  }
+  for_act_dtype(x, [&](auto t) { bwd_impl<typename decltype(t)::type>(dy, mask, x, saved, work, weight, dx, dres, dw, db, relu, write_res, sync); });
   return {dx, dres, dw, db};
 }
 
@@ -705,34 +697,17 @@ static void bwd2_impl(const at::Tensor& dya, const at::Tensor& dyb, const at::Te
                       const SyncBN* sync) {
   const Geometry g = geometry(x);
   cudaStream_t st = at::cuda::getCurrentCUDAStream();
-  const T* ap = reinterpret_cast<const T*>(dya.data_ptr());
-  const T* bp = reinterpret_cast<const T*>(dyb.data_ptr());
-  const uint8_t* mk = relu ? mask.data_ptr<uint8_t>() : nullptr;
-  const T* xp = reinterpret_cast<const T*>(x.data_ptr());
   T* gp = reinterpret_cast<T*>(g_out.data_ptr());
-  float* wk = work.data_ptr<float>();
-  const float* sv = saved.data_ptr<float>();
+  const auto reduce = relu ? bn_bwd_reduce_sum_kernel<T, true> : bn_bwd_reduce_sum_kernel<T, false>;
   int rpb;
-  const int rgrid = reduce_grid(g, &rpb, relu ? resident_ctas(bn_bwd_reduce_sum_kernel<T, true>, g.smem)
-                                             : resident_ctas(bn_bwd_reduce_sum_kernel<T, false>, g.smem));
+  const int rgrid = reduce_grid(g, &rpb, resident_ctas(reduce, g.smem));
   at::Tensor part = partials(x, rgrid, g.C);
-  float* pp = part.data_ptr<float>();
-  if (relu) bn_bwd_reduce_sum_kernel<T, true><<<rgrid, kBnThreads, g.smem, st>>>(ap, bp, mk, xp, sv, gp, pp, g.M, g.C, rpb);
-  else      bn_bwd_reduce_sum_kernel<T, false><<<rgrid, kBnThreads, g.smem, st>>>(ap, bp, mk, xp, sv, gp, pp, g.M, g.C, rpb);
+  reduce<<<rgrid, kBnThreads, g.smem, st>>>(reinterpret_cast<const T*>(dya.data_ptr()), reinterpret_cast<const T*>(dyb.data_ptr()),
+                                            relu ? mask.data_ptr<uint8_t>() : nullptr, reinterpret_cast<const T*>(x.data_ptr()),
+                                            saved.data_ptr<float>(), gp, part.data_ptr<float>(), g.M, g.C, rpb);
   C10_CUDA_KERNEL_LAUNCH_CHECK();
   // second pass: g already carries the mask, and it IS the residual gradient -> the plain (no ReLU, no dres) apply variant
-  if (sync) {
-    sync_bn_exchange(pp, rgrid, g.C, g.M, wk, *sync, st);
-    bn_bwd_apply_sync_kernel<T, false, false><<<apply_grid(g), kBnThreads, 0, st>>>(gp, nullptr, xp, sv, wk + 2 * g.C, w.data_ptr(), wdtype(w),
-                                                                                  reinterpret_cast<T*>(dx.data_ptr()), nullptr, dw.data_ptr(),
-                                                                                  db.data_ptr(), g.M, g.C);
-  } else {
-    combine_partials(pp, rgrid, 2 * g.C, wk, st);
-    bn_bwd_apply_kernel<T, false, false><<<apply_grid(g), kBnThreads, 0, st>>>(gp, nullptr, xp, sv, wk, w.data_ptr(), wdtype(w),
-                                                                             reinterpret_cast<T*>(dx.data_ptr()), nullptr, dw.data_ptr(),
-                                                                             db.data_ptr(), g.M, g.C);
-  }
-  C10_CUDA_KERNEL_LAUNCH_CHECK();
+  bwd_apply<T>(g, part, gp, nullptr, x, saved, work, w, dx, nullptr, dw, db, false, sync, st);
 }
 
 // returns {dx, g = (dy_a + dy_b) * relu_mask (the residual gradient), dweight, dbias}
@@ -752,19 +727,13 @@ std::vector<at::Tensor> bn_act_backward2(const at::Tensor& dy_a_in, const at::Te
     mask = *mask_opt;
   }
   const int C = (int)x.size(1);
-  TORCH_CHECK(work.defined() && work.scalar_type() == at::kFloat && work.numel() >= 2 * C, "work buffer too small");
+  check_work(work, C, sync);
   TORCH_CHECK(saved.defined() && saved.scalar_type() == at::kFloat && saved.numel() >= 2 * C, "saved statistics missing");
   c10::cuda::CUDAGuard guard(x.device());
   at::Tensor g = at::empty_like(x, x.options().memory_format(cl));
   at::Tensor dx = at::empty_like(x, x.options().memory_format(cl));
   at::Tensor dw = at::empty_like(weight), db = at::empty_like(weight);
-  check_sync_work(sync, work, C);
-  switch (x.scalar_type()) {
-    case at::kBFloat16: bwd2_impl<__nv_bfloat16>(dya, dyb, mask, x, saved, work, weight, g, dx, dw, db, relu, sync); break;
-    case at::kHalf: bwd2_impl<__half>(dya, dyb, mask, x, saved, work, weight, g, dx, dw, db, relu, sync); break;
-    case at::kFloat: bwd2_impl<float>(dya, dyb, mask, x, saved, work, weight, g, dx, dw, db, relu, sync); break;
-    default: TORCH_CHECK(false, "unsupported activation dtype");
-  }
+  for_act_dtype(x, [&](auto t) { bwd2_impl<typename decltype(t)::type>(dya, dyb, mask, x, saved, work, weight, g, dx, dw, db, relu, sync); });
   return {dx, g, dw, db};
 }
 
@@ -1139,27 +1108,16 @@ static void stem_fwd_impl(const at::Tensor& x, at::Tensor& y, at::Tensor& code, 
   const Geometry g = geometry(x);
   const PoolGeom pg = pool_geom(x);
   cudaStream_t st = at::cuda::getCurrentCUDAStream();
-  const T* xp = reinterpret_cast<const T*>(x.data_ptr());
-  float* wk = work.defined() ? work.data_ptr<float>() : nullptr;
-  if (training && !stats_ready) {      // stats_ready: the producing GEMM already reduced sum / sum-of-squares into `work`
-    int rpb;
-    const int grid = reduce_grid(g, &rpb, resident_ctas(bn_stats_kernel<T>, g.smem));
-    at::Tensor part = partials(x, grid, g.C);
-    bn_stats_kernel<T><<<grid, kBnThreads, g.smem, st>>>(xp, part.data_ptr<float>(), g.M, g.C, rpb);
-    C10_CUDA_KERNEL_LAUNCH_CHECK();
-    if (sync) sync_bn_exchange(part.data_ptr<float>(), grid, g.C, g.M, wk, *sync, st);
-    else combine_partials(part.data_ptr<float>(), grid, 2 * g.C, wk, st);
-  }
+  const float* sums = forward_sums<T>(x, g, work, training && !stats_ready, sync, st);
   const int cgs = g.C / 8;
   const int64_t total = x.size(0) * pg.OH * pg.OW;
   const int ppb = kBnThreads / cgs;
   const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((total + ppb - 1) / ppb, (int64_t)g.sms * 16));
-  auto kernel = sync ? stem_fwd_sync_kernel<T> : stem_fwd_kernel<T>;
-  kernel<<<grid, kBnThreads, 0, st>>>(xp, reinterpret_cast<T*>(y.data_ptr()), code.defined() ? reinterpret_cast<uint2*>(code.data_ptr()) : nullptr,
-                                      sync ? wk + 2 * g.C : wk, w.data_ptr(), b.data_ptr(), wdtype(w), rm.defined() ? rm.data_ptr<float>() : nullptr,
-                                      rv.defined() ? rv.data_ptr<float>() : nullptr, nbt.defined() ? nbt.data_ptr<int64_t>() : nullptr,
-                                      saved.defined() ? saved.data_ptr<float>() : nullptr, g.M, (int)x.size(0), g.C, pg, eps, momentum,
-                                      training ? 1 : 0);
+  static constexpr decltype(&stem_fwd_kernel<T>) kernels[2] = {stem_fwd_kernel<T>, stem_fwd_sync_kernel<T>};   // [sync]
+  kernels[sync != nullptr]<<<grid, kBnThreads, 0, st>>>(
+      reinterpret_cast<const T*>(x.data_ptr()), reinterpret_cast<T*>(y.data_ptr()), reinterpret_cast<uint2*>(ptr_or_null<uint8_t>(code)), sums,
+      w.data_ptr(), b.data_ptr(), wdtype(w), ptr_or_null<float>(rm), ptr_or_null<float>(rv), ptr_or_null<int64_t>(nbt),
+      ptr_or_null<float>(saved), g.M, (int)x.size(0), g.C, pg, eps, momentum, training ? 1 : 0);
   C10_CUDA_KERNEL_LAUNCH_CHECK();
 }
 
@@ -1180,17 +1138,14 @@ static std::vector<at::Tensor> stem_forward_common(const at::Tensor& x, const at
   at::Tensor saved, code, nbt;
   if (num_batches_tracked.has_value() && num_batches_tracked->defined()) nbt = *num_batches_tracked;
   if (training) {
-    TORCH_CHECK(work.defined() && work.numel() >= 2 * C, "work buffer too small");
+    check_work(work, C, sync);
     saved = at::empty({2 * C}, x.options().dtype(at::kFloat));
   }
   if (need_code) code = at::empty({y.numel()}, x.options().dtype(at::kByte));
-  check_sync_work(sync, work, C);
-  switch (x.scalar_type()) {
-    case at::kBFloat16: stem_fwd_impl<__nv_bfloat16>(x, y, code, work, saved, weight, bias, running_mean, running_var, nbt, training, (float)momentum, (float)eps, stats_ready, sync); break;
-    case at::kHalf: stem_fwd_impl<__half>(x, y, code, work, saved, weight, bias, running_mean, running_var, nbt, training, (float)momentum, (float)eps, stats_ready, sync); break;
-    case at::kFloat: stem_fwd_impl<float>(x, y, code, work, saved, weight, bias, running_mean, running_var, nbt, training, (float)momentum, (float)eps, stats_ready, sync); break;
-    default: TORCH_CHECK(false, "unsupported activation dtype");
-  }
+  for_act_dtype(x, [&](auto t) {
+    stem_fwd_impl<typename decltype(t)::type>(x, y, code, work, saved, weight, bias, running_mean, running_var, nbt, training, (float)momentum,
+                                              (float)eps, stats_ready, sync);
+  });
   return {y, saved, code};
 }
 
@@ -1224,16 +1179,10 @@ static void stem_bwd_impl(const at::Tensor& dp, const at::Tensor& code, const at
   at::Tensor part = partials(x, grid, g.C);
   stem_bwd_reduce_kernel<T><<<grid, kBnThreads, g.smem, st>>>(dpp, cp, xp, saved.data_ptr<float>(), part.data_ptr<float>(), g.M, g.C, pg, rpb);
   C10_CUDA_KERNEL_LAUNCH_CHECK();
-  if (sync) {
-    sync_bn_exchange(part.data_ptr<float>(), grid, g.C, g.M, work.data_ptr<float>(), *sync, st);
-    stem_bwd_apply_sync_kernel<T><<<grid, kBnThreads, 0, st>>>(dpp, cp, xp, saved.data_ptr<float>(), work.data_ptr<float>() + 2 * g.C, w.data_ptr(),
-                                                              wdtype(w), reinterpret_cast<T*>(dx.data_ptr()), dw.data_ptr(), db.data_ptr(), g.M,
-                                                              g.C, pg, rpb);
-  } else {
-    combine_partials(part.data_ptr<float>(), grid, 2 * g.C, work.data_ptr<float>(), st);
-    stem_bwd_apply_kernel<T><<<grid, kBnThreads, 0, st>>>(dpp, cp, xp, saved.data_ptr<float>(), work.data_ptr<float>(), w.data_ptr(), wdtype(w),
-                                                         reinterpret_cast<T*>(dx.data_ptr()), dw.data_ptr(), db.data_ptr(), g.M, g.C, pg, rpb);
-  }
+  const float* sums = finish_sums(part.data_ptr<float>(), grid, g.C, g.M, work.data_ptr<float>(), sync, st);
+  static constexpr decltype(&stem_bwd_apply_kernel<T>) kernels[2] = {stem_bwd_apply_kernel<T>, stem_bwd_apply_sync_kernel<T>};   // [sync]
+  kernels[sync != nullptr]<<<grid, kBnThreads, 0, st>>>(dpp, cp, xp, saved.data_ptr<float>(), sums, w.data_ptr(), wdtype(w),
+                                                        reinterpret_cast<T*>(dx.data_ptr()), dw.data_ptr(), db.data_ptr(), g.M, g.C, pg, rpb);
   C10_CUDA_KERNEL_LAUNCH_CHECK();
 }
 
@@ -1244,17 +1193,11 @@ std::vector<at::Tensor> stem_backward(const at::Tensor& dp_in, const at::Tensor&
   at::Tensor dp = dp_in.is_contiguous(at::MemoryFormat::ChannelsLast) ? dp_in : dp_in.contiguous(at::MemoryFormat::ChannelsLast);
   const int C = (int)x.size(1);
   TORCH_CHECK(dp.scalar_type() == x.scalar_type() && dp.size(1) == C && code.scalar_type() == at::kByte && code.numel() == dp.numel());
-  TORCH_CHECK(work.defined() && work.numel() >= 2 * C, "work buffer too small");
-  check_sync_work(sync, work, C);
+  check_work(work, C, sync);
   c10::cuda::CUDAGuard guard(x.device());
   at::Tensor dx = at::empty_like(x, x.options().memory_format(at::MemoryFormat::ChannelsLast));
   at::Tensor dw = at::empty_like(weight), db = at::empty_like(weight);
-  switch (x.scalar_type()) {
-    case at::kBFloat16: stem_bwd_impl<__nv_bfloat16>(dp, code, x, saved, work, weight, dx, dw, db, sync); break;
-    case at::kHalf: stem_bwd_impl<__half>(dp, code, x, saved, work, weight, dx, dw, db, sync); break;
-    case at::kFloat: stem_bwd_impl<float>(dp, code, x, saved, work, weight, dx, dw, db, sync); break;
-    default: TORCH_CHECK(false, "unsupported activation dtype");
-  }
+  for_act_dtype(x, [&](auto t) { stem_bwd_impl<typename decltype(t)::type>(dp, code, x, saved, work, weight, dx, dw, db, sync); });
   return {dx, dw, db};
 }
 

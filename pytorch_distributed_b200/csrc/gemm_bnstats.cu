@@ -310,8 +310,7 @@ static void launch_gemm(const at::Tensor& a, const at::Tensor& b, at::Tensor& c,
   at::Tensor part = at::empty({ctas_per_n, 2 * N}, gsum.options());
   gemm_bnstats_kernel<T, BLOCK_N><<<grid, kGemmThreads, smem, st>>>(ma, mb, mc, part.data_ptr<float>(), N, K, m_tiles, n_tiles, ctas_per_n);
   C10_CUDA_KERNEL_LAUNCH_CHECK();
-  if (sync) sync_bn_exchange(part.data_ptr<float>(), ctas_per_n, N, M, gsum.data_ptr<float>(), *sync, st);
-  else combine_partials(part.data_ptr<float>(), ctas_per_n, 2 * N, gsum.data_ptr<float>(), st);
+  finish_sums(part.data_ptr<float>(), ctas_per_n, N, M, gsum.data_ptr<float>(), sync, st);
 }
 
 template <typename T>
@@ -334,7 +333,7 @@ at::Tensor conv1x1_bnstats(const at::Tensor& x, const at::Tensor& weight, at::Te
   const int64_t M64 = x.size(0) * x.size(2) * x.size(3);
   const int K = (int)x.size(1), N = (int)weight.size(0);
   TORCH_CHECK(weight.size(1) == K && K % kBlockK == 0 && N % 64 == 0 && M64 < (int64_t)1 << 31, "conv1x1_bnstats: unsupported shape");
-  TORCH_CHECK(gsum.scalar_type() == at::kFloat && gsum.numel() >= (sync ? kSyncWork(N) : 2 * N) && gsum.is_contiguous());
+  check_work(gsum, N, sync);
   TORCH_CHECK((reinterpret_cast<uintptr_t>(x.data_ptr()) & 15) == 0, "x must be 16-byte aligned");
   c10::cuda::CUDAGuard guard(x.device());
   at::Tensor w2 = weight.reshape({N, K}).contiguous();       // [N, K] K-major (a view for both NCHW and NHWC 1x1 weights)

@@ -74,6 +74,13 @@ constexpr int64_t kSyncWork(int64_t C) { return 4 * C + 4; }
 // then every rank publishes them with its row count and work[2C:4C] / work[4C:4C+2] receive the rank-order global sums
 // and the global count.
 void sync_bn_exchange(const float* part, int nblocks, int C, int64_t rows, float* work, const SyncBN& s, cudaStream_t st);
+// `work` is a float work slice of one direction of a C-channel layer: [2C], or [kSyncWork(C)] with a handle
+void check_work(const at::Tensor& work, int64_t C, const SyncBN* sync);
+// Where an apply kernel reads its sums in a work slice: the global sums with a handle, else this rank's
+float* work_sums(float* work, int C, const SyncBN* sync);
+// The reduction step after every pass that wrote per-CTA partials: sync_bn_exchange with a handle, else combine_partials.
+// Returns work_sums(work, C, sync).
+float* finish_sums(const float* part, int nblocks, int C, int64_t rows, float* work, const SyncBN* sync, cudaStream_t st);
 
 // ---- gemm_bnstats.cu (wgmma / TMA)
 at::Tensor conv1x1_bnstats(const at::Tensor& x, const at::Tensor& weight, at::Tensor gsum, const SyncBN* sync);

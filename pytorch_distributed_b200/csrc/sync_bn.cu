@@ -106,4 +106,17 @@ void sync_bn_exchange(const float* part, int nblocks, int C, int64_t rows, float
   C10_CUDA_KERNEL_LAUNCH_CHECK();
 }
 
+void check_work(const at::Tensor& work, int64_t C, const SyncBN* sync) {
+  TORCH_CHECK(work.defined() && work.scalar_type() == at::kFloat && work.is_contiguous() && work.numel() >= 2 * C, "work buffer too small");
+  TORCH_CHECK(!sync || work.numel() >= kSyncWork(C), "synchronised BatchNorm needs a work slice of ", kSyncWork(C), " floats");
+}
+
+float* work_sums(float* work, int C, const SyncBN* sync) { return sync ? work + 2 * C : work; }
+
+float* finish_sums(const float* part, int nblocks, int C, int64_t rows, float* work, const SyncBN* sync, cudaStream_t st) {
+  if (sync) sync_bn_exchange(part, nblocks, C, rows, work, *sync, st);
+  else combine_partials(part, nblocks, 2 * C, work, st);
+  return work_sums(work, C, sync);
+}
+
 }  // namespace ptd

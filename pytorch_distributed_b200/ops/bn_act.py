@@ -18,7 +18,7 @@ from typing import Optional
 import torch
 import torch.nn.functional as F
 
-from .sync_bn import work_len
+from .sync_bn import effective, kernel_arg, work_len
 
 
 def bn_act_reference(x, weight, bias, running_mean, running_var, residual=None, relu=True, training=True, momentum=0.1,
@@ -52,6 +52,26 @@ class _Workspace:
         s = self.buf[self.used: self.used + n]
         self.used += n
         return s, self.generation
+
+    def layer(self, c: int, sync) -> "_LayerWork":
+        """The accumulator slices of one fused BatchNorm layer of ``c`` channels: ``work_len(c, sync)`` floats per direction."""
+        wl = work_len(c, sync)
+        work, gen = self.take(2 * wl)
+        return _LayerWork(self, work, gen, wl)
+
+
+class _LayerWork:
+    """``fwd``: the slice the forward (or the GEMM producing its statistics) accumulates into; ``bwd()``: the backward's."""
+
+    def __init__(self, ws, work, gen, wl):
+        self.fwd = work[:wl]
+        self._bwd = work[wl:]
+        self._ws, self._gen, self._wl = ws, gen, wl
+
+    def bwd(self):
+        if self._gen != -1 and self._gen != self._ws.generation:     # slice was recycled: use a fresh one
+            return torch.zeros(self._wl, dtype=torch.float32, device=self._bwd.device)
+        return self._bwd
 
 
 _workspaces = {}
@@ -186,26 +206,16 @@ class _BnActFn(torch.autograd.Function):
         from .. import _ext
         C = _kernels(x)
         ctx.set_materialize_grads(False)
-        nc = x.size(1)
-        ws = workspace(x.device)
-        wl = work_len(nc, sync)
-        stats_ready = pre is not None          # (work[2 wl], generation): sums already reduced by the producing GEMM
-        if stats_ready:
-            work, gen = pre
-        elif training:
-            work, gen = ws.take(2 * wl)
-        else:
-            work, gen = torch.empty(0, dtype=torch.float32, device=x.device), -1
+        stats_ready = pre is not None          # the layer's slices: sums already reduced by the producing GEMM
+        lw = pre if stats_ready else (workspace(x.device).layer(x.size(1), sync) if training else None)
         _ext.note_launch(1 if (stats_ready or not training) else 3)   # stats + combine (or exchange) + apply
         y, saved, mask = C.bn_act_forward(x, residual, weight, bias, running_mean, running_var, nbt, training, momentum, eps, relu,
-                                          need_grad, work[:wl] if training else work, stats_ready,
-                                          None if sync is None else sync.kernel_arg(C))
+                                          need_grad, lw.fwd if training else torch.empty(0, dtype=torch.float32, device=x.device),
+                                          stats_ready, kernel_arg(sync, C))
         ctx.relu = relu
         ctx.has_res = residual is not None
         ctx.sync = sync
-        ctx.work = work[wl:] if training else None
-        ctx.gen = gen
-        ctx.ws = ws
+        ctx.work = lw
         if need_grad:
             if not training:
                 raise RuntimeError("fused bn_act: backward through eval-mode batch norm is not supported")
@@ -224,12 +234,9 @@ class _BnActFn(torch.autograd.Function):
             return (None, None, None, None) + none
         x, mask, weight, saved = ctx.saved_tensors
         C = _kernels(x)
-        work = ctx.work
-        sync = ctx.sync
-        if work is None or (ctx.gen != -1 and ctx.gen != ctx.ws.generation):
-            work = torch.zeros(work_len(x.size(1), sync), dtype=torch.float32, device=x.device)   # slice was recycled: use a fresh one
+        work = ctx.work.bwd()
         _ext.note_launch(3)                     # reduce + combine (or exchange) + apply
-        karg = None if sync is None else sync.kernel_arg(C)
+        karg = kernel_arg(ctx.sync, C)
         if dy2 is not None:                     # add + mask + reductions in one pass; g doubles as the residual gradient
             dx, dres, dw, db = C.bn_act_backward2(dy, dy2, x, mask, weight, saved, ctx.relu, work, karg)
         else:
@@ -253,10 +260,8 @@ def bn_act(x, weight, bias, running_mean, running_var, residual: Optional[torch.
     ``split=True`` returns the result twice - two aliases of one buffer for the two consumers of a residual block's
     output - so that backward receives their gradients separately and fuses the add (``bn_act_backward2``).
     ``sync``: a ``SyncContext`` of world > 1 synchronises the training-mode statistics over the ranks."""
-    if sync is not None and (not training or sync.world == 1):
-        sync = None
     y = _bn_act(x, weight, bias, running_mean, running_var, residual, relu, training, momentum, eps, fused, num_batches_tracked, split,
-                sync)
+                effective(sync, training))
     if split and not isinstance(y, tuple):
         return y, y
     return y
@@ -313,27 +318,33 @@ def sync_batch_norm_unfused(x, weight, bias, running_mean, running_var, momentum
     return _TorchSyncBN.apply(x, weight, bias, running_mean, running_var, eps, momentum, group, sync.world)
 
 
+def batch_norm_unfused(x, weight, bias, running_mean, running_var, training, momentum, eps, num_batches_tracked, sync, tail):
+    """``tail(batch_norm(x))`` in plain PyTorch, for what the fused kernels cannot take.  ``tail`` is the rest of the op
+    (residual add, ReLU, pooling); it receives the normalised tensor in the dtype the math ran in."""
+    if sync is not None:
+        return tail(sync_batch_norm_unfused(x, weight, bias, running_mean, running_var, momentum, eps, num_batches_tracked, sync))
+    if weight is not None and x.is_cuda and weight.dtype != torch.float32 and x.dtype != weight.dtype:
+        weight, bias = weight.to(x.dtype), bias.to(x.dtype)
+    if training and num_batches_tracked is not None:
+        num_batches_tracked.add_(1)
+    if not x.is_cuda and x.dtype != torch.float32:
+        # CPU batch_norm wants one dtype for activations and statistics: do the math in fp32 (test / debug path)
+        y = F.batch_norm(x.float(), running_mean, running_var, None if weight is None else weight.float(),
+                         None if bias is None else bias.float(), training, momentum, eps)
+        return tail(y).to(x.dtype)
+    return tail(F.batch_norm(x, running_mean, running_var, weight, bias, training, momentum, eps))
+
+
 def _bn_act(x, weight, bias, running_mean, running_var, residual, relu, training, momentum, eps, fused, num_batches_tracked, split,
             sync=None):
     ok = _can_fuse(x, weight, residual, running_mean, emulate=(fused == "emulate"))
     use = ok if fused is None else (bool(fused) and ok)
-    if sync is not None and (not use or (x.is_cuda and sync.native is None)):
-        y = sync_batch_norm_unfused(x, weight, bias, running_mean, running_var, momentum, eps, num_batches_tracked, sync)
-        if residual is not None:
-            y = y + residual
-        return F.relu(y) if relu else y
-    if not use:
-        if weight is not None and x.is_cuda and weight.dtype != torch.float32 and x.dtype != weight.dtype:
-            weight, bias = weight.to(x.dtype), bias.to(x.dtype)
-        if training and num_batches_tracked is not None:
-            num_batches_tracked.add_(1)
-        if not x.is_cuda and x.dtype != torch.float32:
-            # CPU batch_norm wants one dtype for activations and statistics: do the math in fp32 (test / debug path)
-            y = bn_act_reference(x.float(), None if weight is None else weight.float(), None if bias is None else bias.float(),
-                                 running_mean, running_var, None if residual is None else residual.float(), relu, training,
-                                 momentum, eps)
-            return y.to(x.dtype)
-        return bn_act_reference(x, weight, bias, running_mean, running_var, residual, relu, training, momentum, eps)
+    if not use or (sync is not None and x.is_cuda and sync.native is None):
+        def tail(y):
+            if residual is not None:
+                y = y + (residual if y.dtype == x.dtype else residual.to(y.dtype))
+            return F.relu(y) if relu else y
+        return batch_norm_unfused(x, weight, bias, running_mean, running_var, training, momentum, eps, num_batches_tracked, sync, tail)
     need_grad = torch.is_grad_enabled() and (x.requires_grad or weight.requires_grad or bias.requires_grad
                                              or (residual is not None and residual.requires_grad))
     if need_grad and not training:      # backward through frozen (eval-mode) statistics: rare, use the composition

@@ -15,7 +15,7 @@ from __future__ import annotations
 import torch
 
 from .bn_act import _BnActFn, _can_fuse, workspace
-from .sync_bn import work_len
+from .sync_bn import kernel_arg
 
 
 class _Conv1x1Stats(torch.autograd.Function):
@@ -23,7 +23,8 @@ class _Conv1x1Stats(torch.autograd.Function):
     def forward(ctx, x, weight, stats, sync=None):
         from .. import _ext
         _ext.note_launch(2)                     # GEMM + statistics combine (or cross-rank exchange)
-        y = _ext.lib().conv1x1_bnstats(x, weight, stats, sync)
+        C = _ext.lib()
+        y = C.conv1x1_bnstats(x, weight, stats, kernel_arg(sync, C))
         ctx.save_for_backward(x, weight)
         return y
 
@@ -69,17 +70,14 @@ def conv1x1_bn_act(x, conv, bn, residual=None, enabled=True, split=False):
     sync = bn.sync_context()
     if not (enabled and training and can_fuse_conv1x1(x, conv) and bn.fused is not False and (sync is None or sync.native is not None)):
         return bn(conv(x), residual, split) if split else bn(conv(x), residual)
-    nc = conv.weight.size(0)
-    ws = workspace(x.device)
-    wl = work_len(nc, sync)
-    work, gen = ws.take(2 * wl)
-    y = _Conv1x1Stats.apply(x, gemm_weight(conv.weight, autocast_gemm_dtype()), work[:wl], None if sync is None else sync.native)
+    lw = workspace(x.device).layer(conv.weight.size(0), sync)
+    y = _Conv1x1Stats.apply(x, gemm_weight(conv.weight, autocast_gemm_dtype()), lw.fwd, sync)
     if not _can_fuse(y, bn.weight, residual, bn.running_mean):
         return bn(y, residual, split) if split else bn(y, residual)   # (cannot happen for the shapes accepted above)
     need_grad = torch.is_grad_enabled() and (y.requires_grad or bn.weight.requires_grad)
     nbt = bn.num_batches_tracked if (bn.training and bn.track_running_stats) else None
     out = _BnActFn.apply(y, residual, bn.weight, bn.bias, bn.running_mean, bn.running_var, nbt, True,
-                         0.1 if bn.momentum is None else float(bn.momentum), float(bn.eps), bn.relu, need_grad, (work, gen),
+                         0.1 if bn.momentum is None else float(bn.momentum), float(bn.eps), bn.relu, need_grad, lw,
                          bool(split and need_grad), sync)
     if split and not isinstance(out, tuple):
         return out, out

@@ -8,8 +8,8 @@ from __future__ import annotations
 import torch
 import torch.nn.functional as F
 
-from .bn_act import bn_act_reference, sync_batch_norm_unfused, workspace
-from .sync_bn import work_len
+from .bn_act import batch_norm_unfused, bn_act_reference, workspace
+from .sync_bn import effective, kernel_arg
 
 
 def bn_relu_maxpool_reference(x, weight, bias, running_mean, running_var, training=True, momentum=0.1, eps=1e-5):
@@ -19,21 +19,16 @@ def bn_relu_maxpool_reference(x, weight, bias, running_mean, running_var, traini
 
 class _StemFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, x, weight, bias, running_mean, running_var, nbt, training, momentum, eps, need_grad, sync=None):
+    def forward(ctx, x, weight, bias, running_mean, running_var, nbt, training, momentum, eps, need_grad, sync=None, pre=None):
         from .. import _ext
         C = _ext.lib()
-        nc = x.size(1)
-        ws = workspace(x.device)
-        wl = work_len(nc, sync)
-        if training:
-            work, gen = ws.take(2 * wl)
-        else:
-            work, gen = torch.empty(0, dtype=torch.float32, device=x.device), -1
-        _ext.note_launch(3 if training else 1)
-        y, saved, code = C.stem_forward(x, weight, bias, running_mean, running_var, nbt, training, momentum, eps, need_grad,
-                                        work[:wl] if training else work, None if sync is None else sync.native)
-        ctx.work = work[wl:] if training else None
-        ctx.gen, ctx.ws, ctx.sync = gen, ws, sync
+        stats_ready = pre is not None          # the layer's slices: sums already reduced by the producing GEMM (stem_conv.py)
+        lw = pre if stats_ready else (workspace(x.device).layer(x.size(1), sync) if training else None)
+        _ext.note_launch(1 if (stats_ready or not training) else 3)
+        fwd = C.stem_forward_pre if stats_ready else C.stem_forward
+        y, saved, code = fwd(x, weight, bias, running_mean, running_var, nbt, training, momentum, eps, need_grad,
+                             lw.fwd if training else torch.empty(0, dtype=torch.float32, device=x.device), kernel_arg(sync, C))
+        ctx.work, ctx.sync = lw, sync
         if need_grad:
             if not training:
                 raise RuntimeError("fused stem: backward through eval-mode batch norm is not supported")
@@ -45,13 +40,9 @@ class _StemFn(torch.autograd.Function):
         from .. import _ext
         C = _ext.lib()
         x, code, weight, saved = ctx.saved_tensors
-        work = ctx.work
-        sync = ctx.sync
-        if work is None or (ctx.gen != -1 and ctx.gen != ctx.ws.generation):
-            work = torch.zeros(work_len(x.size(1), sync), dtype=torch.float32, device=x.device)
         _ext.note_launch(3)
-        dx, dw, db = C.stem_backward(dy, x, code, weight, saved, work, None if sync is None else sync.native)
-        return dx, dw, db, None, None, None, None, None, None, None, None
+        dx, dw, db = C.stem_backward(dy, x, code, weight, saved, ctx.work.bwd(), kernel_arg(ctx.sync, C))
+        return (dx, dw, db) + (None,) * 9
 
 
 def can_fuse_stem(x, weight, running_mean) -> bool:
@@ -64,24 +55,14 @@ def can_fuse_stem(x, weight, running_mean) -> bool:
 def bn_relu_maxpool(x, weight, bias, running_mean, running_var, training=True, momentum=0.1, eps=1e-5, fused=None,
                     num_batches_tracked=None, sync=None):
     """maxpool(relu(bn(x))); ``sync`` (a ``SyncContext``, see ``ops/sync_bn.py``) synchronises the training statistics."""
-    if sync is not None and (not training or sync.world == 1):
-        sync = None
+    sync = effective(sync, training)
     ok = can_fuse_stem(x, weight, running_mean)
     need_grad = torch.is_grad_enabled() and (x.requires_grad or (weight is not None and weight.requires_grad))
     if need_grad and not training:
         ok = False
     use = ok if fused is None else (fused and ok)
-    if sync is not None and not (use and sync.native is not None):
-        y = sync_batch_norm_unfused(x, weight, bias, running_mean, running_var, momentum, eps, num_batches_tracked, sync)
-        return F.max_pool2d(F.relu(y), kernel_size=3, stride=2, padding=1)
-    if not use:
-        if training and num_batches_tracked is not None:
-            num_batches_tracked.add_(1)
-        if weight is not None and x.is_cuda and weight.dtype != torch.float32 and x.dtype != weight.dtype:
-            weight, bias = weight.to(x.dtype), bias.to(x.dtype)
-        if not x.is_cuda and x.dtype != torch.float32:
-            return bn_relu_maxpool_reference(x.float(), weight.float(), bias.float(), running_mean, running_var, training, momentum,
-                                             eps).to(x.dtype)
-        return bn_relu_maxpool_reference(x, weight, bias, running_mean, running_var, training, momentum, eps)
+    if not use or (sync is not None and sync.native is None):
+        return batch_norm_unfused(x, weight, bias, running_mean, running_var, training, momentum, eps, num_batches_tracked, sync,
+                                  lambda y: F.max_pool2d(F.relu(y), kernel_size=3, stride=2, padding=1))
     return _StemFn.apply(x, weight, bias, running_mean, running_var, num_batches_tracked, training, float(momentum), float(eps), need_grad,
-                         sync)
+                         sync, None)

@@ -21,7 +21,7 @@ import torch
 import torch.nn.functional as F
 
 from .bn_act import workspace
-from .sync_bn import work_len
+from .sync_bn import kernel_arg
 from .conv_bn import GEMM_DTYPES, autocast_gemm_dtype, gemm_weight
 from .stem import _StemFn, bn_relu_maxpool, can_fuse_stem
 
@@ -87,7 +87,7 @@ class _StemConvFn(torch.autograd.Function):
             C = _ext.lib()
             _ext.note_launch(3)                 # im2col + GEMM + statistics combine
             a = C.stem_im2col(x)
-            y = C.conv1x1_bnstats(a, packed.view(packed.size(0), K_PAD, 1, 1), stats, sync)
+            y = C.conv1x1_bnstats(a, packed.view(packed.size(0), K_PAD, 1, 1), stats, kernel_arg(sync, C))
         ctx.save_for_backward(a, weight)
         return y
 
@@ -108,27 +108,6 @@ class _StemConvFn(torch.autograd.Function):
         return None, unpack_stem_weight(dwp, weight), None, None, None
 
 
-class _StemPreFn(torch.autograd.Function):
-    """The fused stem tail (BN + ReLU + MaxPool) when the producing GEMM has already reduced the BN statistics."""
-
-    @staticmethod
-    def forward(ctx, x, weight, bias, running_mean, running_var, nbt, momentum, eps, need_grad, work, gen, sync=None):
-        from .. import _ext
-        wl = work_len(x.size(1), sync)
-        _ext.note_launch(1)
-        y, saved, code = _ext.lib().stem_forward_pre(x, weight, bias, running_mean, running_var, nbt, True, momentum, eps, need_grad,
-                                                     work[:wl], None if sync is None else sync.native)
-        ctx.work = work[wl:]
-        ctx.gen, ctx.ws, ctx.sync = gen, workspace(x.device), sync
-        if need_grad:
-            ctx.save_for_backward(x, code, weight, saved)
-        return y
-
-    @staticmethod
-    def backward(ctx, dy):
-        return _StemFn.backward(ctx, dy) + (None,)
-
-
 def stem_conv_bn_relu_maxpool(x, conv, bn, emulate: bool = False):
     """maxpool(relu(bn(conv7x7(x)))) for the ResNet stem modules ``conv`` (nn.Conv2d) and ``bn`` (BNAct), training mode.
     A synchronised ``bn`` (``SyncBNAct``) exchanges the GEMM's statistics across the ranks."""
@@ -143,13 +122,9 @@ def stem_conv_bn_relu_maxpool(x, conv, bn, emulate: bool = False):
     ac = autocast_gemm_dtype()
     if ac is not None and x.dtype != ac:
         x = x.to(ac)                                                   # keeps channels_last
-    ws = workspace(x.device)
-    wl = work_len(nc, sync)
-    work, gen = ws.take(2 * wl)
-    native = None if sync is None else sync.native
-    y = _StemConvFn.apply(x, gemm_weight(conv.weight, ac), work[:wl], False, native)   # always 5 inputs: backward returns 5 gradients
+    lw = workspace(x.device).layer(nc, sync)
+    y = _StemConvFn.apply(x, gemm_weight(conv.weight, ac), lw.fwd, False, sync)   # always 5 inputs: backward returns 5 gradients
     if not can_fuse_stem(y, bn.weight, bn.running_mean):
         raise RuntimeError("stem GEMM output does not fit the fused stem tail")
     need_grad = torch.is_grad_enabled() and (y.requires_grad or bn.weight.requires_grad)
-    return _StemPreFn.apply(y, bn.weight, bn.bias, bn.running_mean, bn.running_var, nbt, momentum, float(bn.eps), need_grad, work, gen,
-                            sync)
+    return _StemFn.apply(y, bn.weight, bn.bias, bn.running_mean, bn.running_var, nbt, True, momentum, float(bn.eps), need_grad, sync, lw)

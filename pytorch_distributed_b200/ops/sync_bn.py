@@ -25,6 +25,16 @@ def work_len(c: int, sync) -> int:
     return sync_work_len(c) if sync is not None else 2 * c
 
 
+def effective(sync, training: bool):
+    """``sync`` when the layer has something to synchronise (training-mode statistics, more than one rank), else None."""
+    return None if sync is None or not training or sync.world == 1 else sync
+
+
+def kernel_arg(sync, kernels):
+    """The ``sync`` argument of an entry point of the kernel module ``kernels`` (``SyncContext.kernel_arg``; None: unsynchronised)."""
+    return None if sync is None else sync.kernel_arg(kernels)
+
+
 class SyncContext:
     """One per communicator; every synchronised layer of the process shares it (the exchanges run in layer order on
     the compute stream, the same order on every rank)."""

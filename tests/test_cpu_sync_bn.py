@@ -258,3 +258,24 @@ def test_cuda_graph_refused_when_layers_fall_back_to_torch():
         with pytest.raises(ValueError, match="CUDA graph"):
             driver.apply_sync_bn(nn.Sequential(nn.BatchNorm2d(8)), cli.parse_args("distributed", base + extra), driver.Strategy(),
                                  torch.device("cuda"))
+
+
+@pytest.mark.parametrize("sync", [None, object()], ids=["local", "sync"])
+def test_backward_slice_recycled_by_reset_is_replaced(sync):
+    """A backward that runs after ``reset`` handed its slice to the next step accumulates into fresh zeros of its own."""
+    from pytorch_distributed_b200.ops.bn_act import _Workspace
+    from pytorch_distributed_b200.ops.sync_bn import work_len
+    ws, c = _Workspace(torch.device("cpu"), capacity=4096), 64
+    wl = work_len(c, sync)
+    lw = ws.layer(c, sync)
+    assert lw.fwd.data_ptr() == ws.buf.data_ptr() and lw.fwd.numel() == wl
+    kept = lw.bwd()
+    assert kept.data_ptr() == ws.buf[wl:].data_ptr() and kept.numel() >= wl
+    kept.fill_(1.0)
+    ws.reset()
+    fresh = lw.bwd()
+    assert fresh.dtype == torch.float32 and fresh.numel() == wl and not fresh.any()
+    lo, hi = ws.buf.data_ptr(), ws.buf.data_ptr() + 4 * ws.buf.numel()
+    assert not lo <= fresh.data_ptr() < hi
+    fresh.fill_(1.0)
+    assert not ws.buf.any()
