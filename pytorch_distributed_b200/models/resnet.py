@@ -53,7 +53,7 @@ class BNAct(nn.BatchNorm2d):
         training = self.training or not self.track_running_stats
         nbt = self.num_batches_tracked if (self.training and self.track_running_stats) else None   # bumped inside the kernel
         return bn_act(x, self.weight, self.bias, self.running_mean, self.running_var, residual=residual, relu=self.relu,
-                      training=training, momentum=0.1 if self.momentum is None else self.momentum, eps=self.eps, fused=self.fused,
+                      training=training, momentum=self.momentum, eps=self.eps, fused=self.fused,
                       num_batches_tracked=nbt, split=split, sync=self.sync_context())
 
     def sync_context(self):
@@ -81,7 +81,9 @@ class SyncBNAct(BNAct):
     The layer binds to the process's communicator (``utils.dist_ops.set_default_communicator``, registered by this
     package's DDP, apex DDP and ``hvd.init``) at its first training forward with world > 1.  With the fused communicator
     the statistics are exchanged inside the fused BatchNorm kernels (``csrc/sync_bn.cu``); layers those kernels cannot
-    take, and other communicators, run ``torch.nn.SyncBatchNorm``'s autograd function over the process group."""
+    take, and other communicators, run ``torch.nn.SyncBatchNorm``'s autograd function over the process group.  So does
+    ``momentum=None`` (cumulative average) on every communicator, the fused one included: it needs an initialised
+    ``torch.distributed`` process group and cannot be captured in a CUDA graph."""
 
     def __init__(self, num_features, eps=1e-5, momentum=0.1, affine=True, track_running_stats=True, process_group=None, relu=False,
                  fused=None, **kw):
@@ -246,13 +248,14 @@ class ResNet(nn.Module):
         bn = self.bn1
         sync = bn.sync_context()
         if STEM_GEMM and bn.training and torch.is_grad_enabled() and bn.fused is not False and (
-                (can_use_stem_gemm(x, self.conv1) and (sync is None or sync.native is not None)) or bn.fused == "emulate"):
+                (can_use_stem_gemm(x, self.conv1) and (sync is None or sync.native is not None) and bn.momentum is not None)
+                or bn.fused == "emulate"):
             x = stem_conv_bn_relu_maxpool(x, self.conv1, bn, emulate=bn.fused == "emulate")
             x = self.layer4(self.layer3(self.layer2(self.layer1(x))))
             return self.fc(torch.flatten(self.avgpool(_pair(x)[0]), 1))
         nbt = bn.num_batches_tracked if (bn.training and bn.track_running_stats) else None
         x = bn_relu_maxpool(self.conv1(x), bn.weight, bn.bias, bn.running_mean, bn.running_var,   # fused stem tail
-                            training=bn.training or not bn.track_running_stats, momentum=0.1 if bn.momentum is None else bn.momentum,
+                            training=bn.training or not bn.track_running_stats, momentum=bn.momentum,
                             eps=bn.eps, fused=bn.fused, num_batches_tracked=nbt, sync=bn.sync_context())
         x = self.layer4(self.layer3(self.layer2(self.layer1(x))))
         x = _pair(x)[0]               # the last block has a single consumer: its second alias stays unused (gradient None)

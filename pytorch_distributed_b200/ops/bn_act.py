@@ -17,6 +17,7 @@ from typing import Optional
 
 import torch
 import torch.nn.functional as F
+from torch.autograd.function import once_differentiable
 
 from .sync_bn import effective, kernel_arg, work_len
 
@@ -66,12 +67,16 @@ class _LayerWork:
     def __init__(self, ws, work, gen, wl):
         self.fwd = work[:wl]
         self._bwd = work[wl:]
-        self._ws, self._gen, self._wl = ws, gen, wl
+        self._ws, self._gen, self._wl, self._dev = ws, gen, wl, work.device
 
     def bwd(self):
-        if self._gen != -1 and self._gen != self._ws.generation:     # slice was recycled: use a fresh one
-            return torch.zeros(self._wl, dtype=torch.float32, device=self._bwd.device)
-        return self._bwd
+        """The backward's slice, handed out once.  The kernels add their sums into the slice they are given, so a second
+        backward through the same graph (``retain_graph=True``, two ``autograd.grad`` calls, two losses over one trunk)
+        and a backward after ``reset`` recycled the slice get fresh zeros instead."""
+        work, self._bwd = self._bwd, None
+        if work is None or (self._gen != -1 and self._gen != self._ws.generation):
+            return torch.zeros(self._wl, dtype=torch.float32, device=self._dev)
+        return work
 
 
 _workspaces = {}
@@ -95,10 +100,20 @@ class _Emu:
     """Pure PyTorch (fp32 math) stand-in for the ``csrc/bn_act.cu`` entry points, same signatures and tensor contracts
     (channels_last activations seen as a row-major [M, C] matrix, 1 mask byte per 8 channels, ``saved`` = mean | invstd).
     It documents what the kernels compute and lets the CPU tests drive the autograd plumbing of :class:`_BnActFn`
-    (``bn_act(..., fused="emulate")``).  With ``sync`` (a ``SyncContext``) the sums and the row count are added over
-    the ranks with the communicator's ``all_reduce_``."""
+    (``bn_act(..., fused="emulate")``).  Like the kernels, each reduction adds its [2C] sums into ``work[:2C]`` and the
+    statistics and gradients are computed from what the slice then holds.  With ``sync`` (a ``SyncContext``) the sums
+    and the row count are added over the ranks with the communicator's ``all_reduce_``."""
 
     is_emulation = True
+
+    @staticmethod
+    def _accumulate(work, sums):
+        """``work[:2C] += sums``; returns a copy of what the slice holds afterwards (``work`` None: a fresh slice)."""
+        if work is None:
+            return sums.clone()
+        w = work[:sums.numel()]
+        w += sums
+        return w.clone()
 
     @staticmethod
     def _rows(t):
@@ -128,17 +143,12 @@ class _Emu:
         m, c = xr.shape
         n = m                                 # rows the statistics cover
         saved = mask = None
-        if training:
-            if sync is not None:              # E[x^2] - E[x]^2 over the global sums, as the kernels compute it
-                local = work[:2 * c] if stats_ready else torch.cat([xr.sum(0), (xr * xr).sum(0)])
-                g, n = _Emu._global_sums(local, m, sync)
-                mean = g[:c] / n
-                var = (g[c:] / n - mean * mean).clamp_min(0)
-            elif stats_ready:
-                mean = work[:c] / m
-                var = (work[c:2 * c] / m - mean * mean).clamp_min(0)
-            else:
-                mean, var = xr.mean(0), xr.var(0, unbiased=False)
+        if training:                          # E[x^2] - E[x]^2 over the (global) sums, as the kernels compute it
+            sums = work[:2 * c].clone() if stats_ready else _Emu._accumulate(work, torch.cat([xr.sum(0), (xr * xr).sum(0)]))
+            if sync is not None:
+                sums, n = _Emu._global_sums(sums, m, sync)
+            mean = sums[:c] / n
+            var = (sums[c:] / n - mean * mean).clamp_min(0)
             invstd = torch.rsqrt(var + eps)
             saved = torch.cat([mean, invstd])
             if rm is not None:
@@ -159,12 +169,13 @@ class _Emu:
         return _Emu._like(v, x), saved, mask
 
     @staticmethod
-    def _bwd_from_g(g, x, weight, saved, sync=None):
+    def _bwd_from_g(g, x, weight, saved, work, sync=None):
         xr = _Emu._rows(x).float()
         m, c = xr.shape
         mean, invstd = saved[:c], saved[c:]
         xhat = (xr - mean) * invstd
-        sdz, sdzx = g.sum(0), (g * xhat).sum(0)
+        sums = _Emu._accumulate(work, torch.cat([g.sum(0), (g * xhat).sum(0)]))
+        sdz, sdzx = sums[:c], sums[c:]
         gdz, gdzx, n = sdz, sdzx, m
         if sync is not None:              # dx from the global sums; dgamma / dbeta stay this rank's
             tot, n = _Emu._global_sums(torch.cat([sdz, sdzx]), m, sync)
@@ -177,7 +188,7 @@ class _Emu:
         g = _Emu._rows(dy).float()
         if relu:
             g = g * _Emu._unpack(mask, *g.shape)
-        dx, dw, db = _Emu._bwd_from_g(g, x, weight, saved, sync)
+        dx, dw, db = _Emu._bwd_from_g(g, x, weight, saved, work, sync)
         dres = None
         if has_res:
             dres = dy if not relu else _Emu._like(g, x)
@@ -188,7 +199,7 @@ class _Emu:
         g = (_Emu._rows(dy_a).float() + _Emu._rows(dy_b).float()).to(x.dtype).float()      # rounded like an eager add
         if relu:
             g = g * _Emu._unpack(mask, *g.shape)
-        dx, dw, db = _Emu._bwd_from_g(g, x, weight, saved, sync)
+        dx, dw, db = _Emu._bwd_from_g(g, x, weight, saved, work, sync)
         return dx, _Emu._like(g, x), dw, db
 
 
@@ -225,6 +236,7 @@ class _BnActFn(torch.autograd.Function):
         return y
 
     @staticmethod
+    @once_differentiable            # the kernels are not differentiable: a second-order gradient raises instead of being cut
     def backward(ctx, dy, dy2=None):
         from .. import _ext
         none = (None,) * 11
@@ -253,13 +265,14 @@ def _can_fuse(x, weight, residual, running_mean=True, emulate=False) -> bool:
 
 
 def bn_act(x, weight, bias, running_mean, running_var, residual: Optional[torch.Tensor] = None, relu: bool = True,
-           training: bool = True, momentum: float = 0.1, eps: float = 1e-5, fused=None,
+           training: bool = True, momentum: Optional[float] = 0.1, eps: float = 1e-5, fused=None,
            num_batches_tracked: Optional[torch.Tensor] = None, split: bool = False, sync=None):
     """relu(batch_norm(x) + residual).  ``fused=None`` picks the CUDA kernels whenever the layout allows it;
     ``fused="emulate"`` runs the same autograd op over the PyTorch emulation of the kernels (CPU tests).
     ``split=True`` returns the result twice - two aliases of one buffer for the two consumers of a residual block's
     output - so that backward receives their gradients separately and fuses the add (``bn_act_backward2``).
-    ``sync``: a ``SyncContext`` of world > 1 synchronises the training-mode statistics over the ranks."""
+    ``sync``: a ``SyncContext`` of world > 1 synchronises the training-mode statistics over the ranks.
+    ``momentum=None``: cumulative average of the running statistics, as ``torch.nn.BatchNorm2d`` (unfused path)."""
     y = _bn_act(x, weight, bias, running_mean, running_var, residual, relu, training, momentum, eps, fused, num_batches_tracked, split,
                 effective(sync, training))
     if split and not isinstance(y, tuple):
@@ -303,9 +316,7 @@ class _SyncBnCpuFn(torch.autograd.Function):
 def sync_batch_norm_unfused(x, weight, bias, running_mean, running_var, momentum, eps, num_batches_tracked, sync):
     """Layers the fused kernels cannot take (NCHW, C % 8 != 0, ...) and communicators other than the fused one: on CUDA
     ``torch.nn.SyncBatchNorm``'s own autograd function over the communicator's process group, on CPU the same semantics
-    over the communicator's ``all_reduce_``."""
-    if num_batches_tracked is not None:
-        num_batches_tracked.add_(1)
+    over the communicator's ``all_reduce_``.  ``momentum`` is the factor itself (``batch_norm_unfused`` resolves None)."""
     if not x.is_cuda:
         return _SyncBnCpuFn.apply(x, weight, bias, running_mean, running_var, eps, momentum, sync)
     if torch.cuda.is_current_stream_capturing():
@@ -320,13 +331,19 @@ def sync_batch_norm_unfused(x, weight, bias, running_mean, running_var, momentum
 
 def batch_norm_unfused(x, weight, bias, running_mean, running_var, training, momentum, eps, num_batches_tracked, sync, tail):
     """``tail(batch_norm(x))`` in plain PyTorch, for what the fused kernels cannot take.  ``tail`` is the rest of the op
-    (residual add, ReLU, pooling); it receives the normalised tensor in the dtype the math ran in."""
+    (residual add, ReLU, pooling); it receives the normalised tensor in the dtype the math ran in.
+    ``momentum=None`` is ``torch.nn.BatchNorm2d``'s cumulative average: factor 1 / ``num_batches_tracked`` after the
+    increment (a host read of the counter, as torch does), 0 without a counter."""
+    if training and num_batches_tracked is not None:
+        num_batches_tracked.add_(1)
+        if momentum is None:
+            momentum = 1.0 / float(num_batches_tracked)
+    if momentum is None:
+        momentum = 0.0
     if sync is not None:
         return tail(sync_batch_norm_unfused(x, weight, bias, running_mean, running_var, momentum, eps, num_batches_tracked, sync))
     if weight is not None and x.is_cuda and weight.dtype != torch.float32 and x.dtype != weight.dtype:
         weight, bias = weight.to(x.dtype), bias.to(x.dtype)
-    if training and num_batches_tracked is not None:
-        num_batches_tracked.add_(1)
     if not x.is_cuda and x.dtype != torch.float32:
         # CPU batch_norm wants one dtype for activations and statistics: do the math in fp32 (test / debug path)
         y = F.batch_norm(x.float(), running_mean, running_var, None if weight is None else weight.float(),
@@ -339,6 +356,8 @@ def _bn_act(x, weight, bias, running_mean, running_var, residual, relu, training
             sync=None):
     ok = _can_fuse(x, weight, residual, running_mean, emulate=(fused == "emulate"))
     use = ok if fused is None else (bool(fused) and ok)
+    if momentum is None and training:   # cumulative average: its factor depends on num_batches_tracked (a host read)
+        use = False
     if not use or (sync is not None and x.is_cuda and sync.native is None):
         def tail(y):
             if residual is not None:
@@ -347,6 +366,8 @@ def _bn_act(x, weight, bias, running_mean, running_var, residual, relu, training
         return batch_norm_unfused(x, weight, bias, running_mean, running_var, training, momentum, eps, num_batches_tracked, sync, tail)
     need_grad = torch.is_grad_enabled() and (x.requires_grad or weight.requires_grad or bias.requires_grad
                                              or (residual is not None and residual.requires_grad))
+    if momentum is None:                # eval mode: the factor is not used
+        momentum = 0.0
     if need_grad and not training:      # backward through frozen (eval-mode) statistics: rare, use the composition
         return bn_act_reference(x, weight.to(x.dtype) if weight.dtype != torch.float32 else weight,
                                 bias.to(x.dtype) if bias.dtype != torch.float32 else bias, running_mean, running_var, residual, relu,

@@ -13,6 +13,7 @@ odd shapes, ``PTD_FUSED_CONV1X1=0`` - runs ``F.conv2d`` + :func:`bn_act`.
 from __future__ import annotations
 
 import torch
+from torch.autograd.function import once_differentiable
 
 from .bn_act import _BnActFn, _can_fuse, workspace
 from .sync_bn import kernel_arg
@@ -29,6 +30,7 @@ class _Conv1x1Stats(torch.autograd.Function):
         return y
 
     @staticmethod
+    @once_differentiable
     def backward(ctx, dy):
         x, weight = ctx.saved_tensors
         dy = dy.contiguous(memory_format=torch.channels_last)
@@ -68,7 +70,8 @@ def conv1x1_bn_act(x, conv, bn, residual=None, enabled=True, split=False):
     A synchronised ``bn`` (``SyncBNAct``) exchanges the GEMM's statistics across the ranks before the apply pass."""
     training = bn.training or not bn.track_running_stats
     sync = bn.sync_context()
-    if not (enabled and training and can_fuse_conv1x1(x, conv) and bn.fused is not False and (sync is None or sync.native is not None)):
+    if not (enabled and training and can_fuse_conv1x1(x, conv) and bn.fused is not False and (sync is None or sync.native is not None)
+            and bn.momentum is not None):       # momentum=None (cumulative average) runs the unfused BatchNorm
         return bn(conv(x), residual, split) if split else bn(conv(x), residual)
     lw = workspace(x.device).layer(conv.weight.size(0), sync)
     y = _Conv1x1Stats.apply(x, gemm_weight(conv.weight, autocast_gemm_dtype()), lw.fwd, sync)
@@ -77,7 +80,7 @@ def conv1x1_bn_act(x, conv, bn, residual=None, enabled=True, split=False):
     need_grad = torch.is_grad_enabled() and (y.requires_grad or bn.weight.requires_grad)
     nbt = bn.num_batches_tracked if (bn.training and bn.track_running_stats) else None
     out = _BnActFn.apply(y, residual, bn.weight, bn.bias, bn.running_mean, bn.running_var, nbt, True,
-                         0.1 if bn.momentum is None else float(bn.momentum), float(bn.eps), bn.relu, need_grad, lw,
+                         float(bn.momentum), float(bn.eps), bn.relu, need_grad, lw,
                          bool(split and need_grad), sync)
     if split and not isinstance(out, tuple):
         return out, out

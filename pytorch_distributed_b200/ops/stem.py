@@ -7,6 +7,7 @@ from __future__ import annotations
 
 import torch
 import torch.nn.functional as F
+from torch.autograd.function import once_differentiable
 
 from .bn_act import batch_norm_unfused, bn_act_reference, workspace
 from .sync_bn import effective, kernel_arg
@@ -36,6 +37,7 @@ class _StemFn(torch.autograd.Function):
         return y
 
     @staticmethod
+    @once_differentiable
     def backward(ctx, dy):
         from .. import _ext
         C = _ext.lib()
@@ -61,8 +63,12 @@ def bn_relu_maxpool(x, weight, bias, running_mean, running_var, training=True, m
     if need_grad and not training:
         ok = False
     use = ok if fused is None else (fused and ok)
+    if momentum is None and training:   # cumulative average (see batch_norm_unfused)
+        use = False
     if not use or (sync is not None and sync.native is None):
         return batch_norm_unfused(x, weight, bias, running_mean, running_var, training, momentum, eps, num_batches_tracked, sync,
                                   lambda y: F.max_pool2d(F.relu(y), kernel_size=3, stride=2, padding=1))
+    if momentum is None:                # eval mode: the factor is not used
+        momentum = 0.0
     return _StemFn.apply(x, weight, bias, running_mean, running_var, num_batches_tracked, training, float(momentum), float(eps), need_grad,
                          sync, None)

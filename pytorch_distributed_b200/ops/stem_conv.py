@@ -19,6 +19,7 @@ from __future__ import annotations
 
 import torch
 import torch.nn.functional as F
+from torch.autograd.function import once_differentiable
 
 from .bn_act import workspace
 from .sync_bn import kernel_arg
@@ -92,6 +93,7 @@ class _StemConvFn(torch.autograd.Function):
         return y
 
     @staticmethod
+    @once_differentiable
     def backward(ctx, dy):
         a, weight = ctx.saved_tensors
         co = weight.size(0)
@@ -112,13 +114,16 @@ def stem_conv_bn_relu_maxpool(x, conv, bn, emulate: bool = False):
     """maxpool(relu(bn(conv7x7(x)))) for the ResNet stem modules ``conv`` (nn.Conv2d) and ``bn`` (BNAct), training mode.
     A synchronised ``bn`` (``SyncBNAct``) exchanges the GEMM's statistics across the ranks."""
     nc = conv.weight.size(0)
-    momentum = 0.1 if bn.momentum is None else float(bn.momentum)
+    momentum = bn.momentum
     nbt = bn.num_batches_tracked if (bn.training and bn.track_running_stats) else None
     sync = bn.sync_context()
     if emulate:                                                        # CPU / test path: same op graph, PyTorch math
         y = _StemConvFn.apply(x, conv.weight, None, True)
         return bn_relu_maxpool(y, bn.weight, bn.bias, bn.running_mean, bn.running_var, training=True, momentum=momentum, eps=bn.eps,
                                fused=False, num_batches_tracked=nbt, sync=sync)
+    if momentum is None:                                               # cumulative average: cuDNN + the unfused BatchNorm
+        return bn_relu_maxpool(conv(x), bn.weight, bn.bias, bn.running_mean, bn.running_var, training=True, momentum=None,
+                               eps=bn.eps, fused=False, num_batches_tracked=nbt, sync=sync)
     ac = autocast_gemm_dtype()
     if ac is not None and x.dtype != ac:
         x = x.to(ac)                                                   # keeps channels_last
@@ -127,4 +132,5 @@ def stem_conv_bn_relu_maxpool(x, conv, bn, emulate: bool = False):
     if not can_fuse_stem(y, bn.weight, bn.running_mean):
         raise RuntimeError("stem GEMM output does not fit the fused stem tail")
     need_grad = torch.is_grad_enabled() and (y.requires_grad or bn.weight.requires_grad)
-    return _StemFn.apply(y, bn.weight, bn.bias, bn.running_mean, bn.running_var, nbt, True, momentum, float(bn.eps), need_grad, sync, lw)
+    return _StemFn.apply(y, bn.weight, bn.bias, bn.running_mean, bn.running_var, nbt, True, float(momentum), float(bn.eps), need_grad,
+                         sync, lw)

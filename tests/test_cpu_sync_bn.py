@@ -57,6 +57,11 @@ for mode in ("emulate", False):
         x = x.contiguous(memory_format=torch.channels_last)
     x.requires_grad_(True)
     y = layer(x)
+    if mode == "emulate":                        # backwards through a retained graph: each exchanges fresh sums, same bits
+        l = (y.double() * dyg[lo:hi]).sum()
+        g1 = torch.autograd.grad(l, [x, layer.weight, layer.bias], retain_graph=True)
+        g2 = torch.autograd.grad(l, [x, layer.weight, layer.bias], retain_graph=True)
+        assert all(torch.equal(a, b) for a, b in zip(g1, g2)), "rank %d: the second backward differs from the first" % r
     (y.double() * dyg[lo:hi]).sum().backward()
     close(y, y_ref[lo:hi], "y")
     close(x.grad, dx_ref, "dx")
