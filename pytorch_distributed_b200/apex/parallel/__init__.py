@@ -16,6 +16,7 @@ from ...parallel.comm import make_communicator
 from ...parallel.ddp import GradientEngine, _float_buffers, sync_module_states
 from ...utils.dist_ops import register_for_sync_batchnorm
 from ...models.resnet import SyncBNAct, convert_sync_batchnorm
+from .LARC import LARC  # noqa: F401  (apex.parallel.LARC; the submodule stays importable as apex.parallel.LARC)
 
 _WIRE = {torch.float16: "fp16", torch.bfloat16: "bf16", torch.float32: "fp32"}
 

@@ -11,6 +11,7 @@ and fall back to $LOCAL_RANK; ``-j/--workers`` is honoured.
 from __future__ import annotations
 
 import argparse
+import math
 import os
 
 
@@ -87,6 +88,15 @@ def build_parser(entry: str = "distributed") -> argparse.ArgumentParser:
     x.add_argument("--no-fused-bn", dest="fused_bn", action="store_false")
     x.add_argument("--optimizer", default="fused", choices=["fused", "torch"],
                    help="fused = hand-written multi-tensor SGD kernel; torch = torch.optim.SGD")
+    x.add_argument("--larc", action="store_true",
+                   help="layer-wise adaptive rates (apex.parallel.LARC) around the optimizer; fused into the SGD kernels with "
+                        "--optimizer fused")
+    x.add_argument("--larc-trust-coefficient", default=None, type=_positive_float, metavar="T",
+                   help="LARC trust coefficient (default: 0.02, apex's)")
+    x.add_argument("--larc-clip", dest="larc_clip", action="store_true", default=None,
+                   help="LARC clip mode: the adaptive factor is min(f / lr, 1) (default)")
+    x.add_argument("--no-larc-clip", dest="larc_clip", action="store_false",
+                   help="LARC scale mode: the gradient is multiplied by f itself")
     x.add_argument("--cuda-graph", action="store_true", help="capture the train step in a CUDA graph")
     x.add_argument("--sync-bn", action="store_true",
                    help="synchronise BatchNorm statistics across the data-parallel ranks (torch.nn.SyncBatchNorm semantics; "
@@ -115,7 +125,21 @@ def resolve_local_rank(args) -> int:
     return lr
 
 
+def _positive_float(s: str) -> float:
+    v = float(s)
+    if not (v > 0 and math.isfinite(v)):
+        raise argparse.ArgumentTypeError("must be a positive finite number, got %r" % (s,))
+    return v
+
+
 def parse_args(entry: str, argv=None):
-    args = build_parser(entry).parse_args(argv)
+    parser = build_parser(entry)
+    args = parser.parse_args(argv)
+    if not args.larc and (args.larc_trust_coefficient is not None or args.larc_clip is not None):
+        parser.error("--larc-trust-coefficient / --larc-clip / --no-larc-clip need --larc")
+    if args.larc_trust_coefficient is None:
+        args.larc_trust_coefficient = 0.02
+    if args.larc_clip is None:
+        args.larc_clip = True
     args.entry = entry
     return args

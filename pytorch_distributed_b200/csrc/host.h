@@ -39,6 +39,14 @@ void fused_sgd_multi(std::vector<at::Tensor> grads, std::vector<at::Tensor> para
 void multi_tensor_scale(std::vector<at::Tensor> src, std::vector<at::Tensor> dst, double scale, at::Tensor found_inf);
 void multi_tensor_axpby(std::vector<at::Tensor> x, std::vector<at::Tensor> y, std::vector<at::Tensor> out, double a, double b,
                         at::Tensor found_inf);
+// LARC: norm pass + SGD update (flat: chunks [chunk_lo, chunk_hi) of a table built once per layout; multi: whole lists)
+constexpr int64_t kLarcChunkElems = 8192;
+void larc_sgd_flat(at::Tensor grad, at::Tensor master, at::Tensor momentum, c10::optional<at::Tensor> model_copy, at::Tensor hyper,
+                   c10::optional<at::Tensor> found_inf, bool nesterov, bool first_step, at::Tensor chunk_tensor, at::Tensor info,
+                   int64_t chunk_lo, int64_t chunk_hi, at::Tensor partials, at::Tensor stats, double trust, double eps, bool clip);
+void larc_sgd_multi(std::vector<at::Tensor> grads, std::vector<at::Tensor> params, std::vector<at::Tensor> momenta,
+                    std::vector<c10::optional<at::Tensor>> model_copies, at::Tensor hyper, c10::optional<at::Tensor> found_inf, bool nesterov,
+                    std::vector<bool> first, std::vector<int64_t> rows, at::Tensor stats, double trust, double eps, bool clip);
 void amp_update_scale(at::Tensor scale, at::Tensor growth_tracker, at::Tensor found_inf, double growth, double backoff,
                       int64_t interval, at::Tensor hyper);
 

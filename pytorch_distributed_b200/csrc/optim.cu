@@ -192,13 +192,15 @@ static uint8_t dtype_code(const at::Tensor& t) {
   }
 }
 
+// launch(a, nb, src): src[slot] is the index in `lists` of the tensor registered in that slot of `a`
 template <int DEPTH, typename LaunchFn>
 static void mta_for_each(const std::vector<std::vector<at::Tensor>>& lists, LaunchFn&& launch) {
   const size_t n = lists[0].size();
   MtaArgs<DEPTH> a;
+  int src[kMtaTensors];
   int nt = 0, nb = 0;
   auto flush = [&]() {
-    if (nb > 0) launch(a, nb);
+    if (nb > 0) launch(a, nb, static_cast<const int*>(src));
     nt = 0;
     nb = 0;
   };
@@ -217,6 +219,7 @@ static void mta_for_each(const std::vector<std::vector<at::Tensor>>& lists, Laun
         a.dtype[d][nt] = dtype_code(lists[d][i]);
       }
       a.numel[nt] = numel;
+      src[nt] = (int)i;
       while (c < chunks && nb < kMtaBlocks) {
         a.block_tensor[nb] = (uint8_t)nt;
         a.block_chunk[nb] = (int32_t)c;
@@ -242,7 +245,7 @@ void fused_sgd_multi(std::vector<at::Tensor> grads, std::vector<at::Tensor> para
   cudaStream_t st = at::cuda::getCurrentCUDAStream();
   const int* fi = found_inf.has_value() ? reinterpret_cast<const int*>(found_inf->data_ptr()) : nullptr;
   const float* hp = hyper.data_ptr<float>();
-  mta_for_each<4>({grads, params, momenta, model_copies}, [&](const MtaArgs<4>& a, int nb) {
+  mta_for_each<4>({grads, params, momenta, model_copies}, [&](const MtaArgs<4>& a, int nb, const int*) {
     fused_sgd_multi_kernel<<<nb, 256, 0, st>>>(a, hp, fi, nesterov, first_step);
     C10_CUDA_KERNEL_LAUNCH_CHECK();
   });
@@ -254,7 +257,7 @@ void multi_tensor_scale(std::vector<at::Tensor> src, std::vector<at::Tensor> dst
   TORCH_CHECK(found_inf.scalar_type() == at::kInt && found_inf.numel() >= 1);
   c10::cuda::CUDAGuard guard(src[0].device());
   cudaStream_t st = at::cuda::getCurrentCUDAStream();
-  mta_for_each<2>({src, dst}, [&](const MtaArgs<2>& a, int nb) {
+  mta_for_each<2>({src, dst}, [&](const MtaArgs<2>& a, int nb, const int*) {
     multi_tensor_scale_kernel<<<nb, 256, 0, st>>>(a, (float)scale, found_inf.data_ptr<int>());
     C10_CUDA_KERNEL_LAUNCH_CHECK();
   });
@@ -267,8 +270,363 @@ void multi_tensor_axpby(std::vector<at::Tensor> x, std::vector<at::Tensor> y, st
   TORCH_CHECK(found_inf.scalar_type() == at::kInt && found_inf.numel() >= 1);
   c10::cuda::CUDAGuard guard(x[0].device());
   cudaStream_t st = at::cuda::getCurrentCUDAStream();
-  mta_for_each<3>({x, y, out}, [&](const MtaArgs<3>& args, int nb) {
+  mta_for_each<3>({x, y, out}, [&](const MtaArgs<3>& args, int nb, const int*) {
     multi_tensor_axpby_kernel<<<nb, 256, 0, st>>>(args, (float)a, (float)b, found_inf.data_ptr<int>());
+    C10_CUDA_KERNEL_LAUNCH_CHECK();
+  });
+}
+
+// ---------------------------------------------------------------- LARC layer-wise adaptive rates (apex.parallel.LARC)
+// Per parameter tensor p with unscaled gradient g = grad * gmul, wd = hyper[2], lr = hyper[0]:
+//   pn = ||p||, gn = ||g||;  if pn != 0 and gn != 0:  f = trust * pn / (gn + pn * wd + eps), clip: f = min(f / lr, 1),
+//   g = (g + wd * p) * f;  otherwise g is left as is and gets no weight decay (apex);  then sgd_update with wd = 0.
+// Two passes, one CTA per kLarcChunk-element chunk of one tensor (chunks counted from the tensor's first element):
+//   larc_norm_*  writes the chunk's fp32 partial sums {sum p^2, sum g^2} to partials[cbase + chunk];
+//   larc_sgd_*   adds its tensor's partials in ascending chunk order, forms pn, gn, f and applies the update; chunk 0 of
+//                each tensor writes {pn, gn, f} to stats[row] (f = 1 where a norm is zero).
+// Within a chunk thread i adds elements 8 (i + 256 k) + j, j = 0..7 then k ascending, and the CTA combines the 256
+// thread sums in a fixed tree.  No float atomics: the flat, per-bucket and multi-tensor front ends give the same bits.
+// HBM traffic per element (bf16 gradient, bf16 copy): 6 B norm pass + the 20 B of the SGD update.
+constexpr int kLarcChunk = kMtaChunk;  // the multi-tensor front end's chunk: its block_chunk is the LARC chunk
+constexpr int kLarcThreads = 256;
+static_assert(kLarcChunk == kLarcChunkElems, "host.h publishes the LARC chunk size");
+static_assert(kLarcChunk % (8 * kLarcThreads) == 0, "a chunk is a whole number of 8-element groups per thread");
+
+struct LarcFactor { float pn, gn, f; bool adapt; };
+
+// per-tensor data of a multi-tensor launch, by slot: first partial, statistics row, first-step flag
+struct LarcSlots {
+  int32_t cbase[kMtaTensors];
+  int32_t row[kMtaTensors];
+  uint8_t first[kMtaTensors];
+};
+
+__device__ __forceinline__ float ldcg_f(const float* p) { return __ldcg(p); }
+__device__ __forceinline__ float ldcg_f(const __nv_bfloat16* p) { return __bfloat162float(__ldcg(p)); }
+__device__ __forceinline__ float ldcg_f(const __half* p) { return __half2float(__ldcg(p)); }
+
+// the one summation order of every front end: elements j < cnt of one 8-element group
+__device__ __forceinline__ void larc_acc8(const float (&p)[8], const float (&g)[8], float gmul, int cnt, float& sp, float& sg) {
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    if (j < cnt) {
+      sp = __fmaf_rn(p[j], p[j], sp);
+      const float u = __fmul_rn(g[j], gmul);
+      sg = __fmaf_rn(u, u, sg);
+    }
+  }
+}
+
+// CTA sum of (a, b) in a fixed order: butterfly within each warp, then warp 0 over the warp totals.  Valid in thread 0.
+__device__ __forceinline__ float2 larc_cta_sum(float a, float b) {
+  __shared__ float2 red[kLarcThreads / 32];
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    a = __fadd_rn(a, __shfl_xor_sync(0xffffffffu, a, o));
+    b = __fadd_rn(b, __shfl_xor_sync(0xffffffffu, b, o));
+  }
+  const int w = threadIdx.x >> 5, l = threadIdx.x & 31;
+  if (l == 0) red[w] = make_float2(a, b);
+  __syncthreads();
+  if (w == 0) {
+    const float2 v = l < kLarcThreads / 32 ? red[l] : make_float2(0.f, 0.f);
+    a = v.x;
+    b = v.y;
+#pragma unroll
+    for (int o = kLarcThreads / 64; o > 0; o >>= 1) {
+      a = __fadd_rn(a, __shfl_xor_sync(0xffffffffu, a, o));
+      b = __fadd_rn(b, __shfl_xor_sync(0xffffffffu, b, o));
+    }
+  }
+  return make_float2(a, b);
+}
+
+__device__ __forceinline__ LarcFactor larc_factor(const float2* part, int64_t nchunks, const SgdHyper& h, float trust, float eps, bool clip) {
+  float sp = 0.f, sg = 0.f;
+  for (int64_t c = 0; c < nchunks; ++c) {
+    const float2 v = part[c];
+    sp = __fadd_rn(sp, v.x);
+    sg = __fadd_rn(sg, v.y);
+  }
+  LarcFactor r;
+  r.pn = __fsqrt_rn(sp);
+  r.gn = __fsqrt_rn(sg);
+  r.adapt = r.pn != 0.f && r.gn != 0.f;
+  r.f = 1.f;
+  if (r.adapt) {
+    r.f = __fdiv_rn(__fmul_rn(trust, r.pn), __fadd_rn(__fmaf_rn(r.pn, h.wd, r.gn), eps));
+    if (clip) r.f = fminf(__fdiv_rn(r.f, h.lr), 1.f);
+  }
+  return r;
+}
+
+// Not inlined: the compiler may contract sgd_update's products into FMAs differently in different callers, and the flat
+// and multi-tensor kernels must give the same bits.  One compiled body serves both; scalar arguments and a float2 result
+// {p, m} keep the call in registers (no addressable arguments, so nothing goes through local memory).
+__device__ __noinline__ float2 larc_update(float g, float p, float m, float f, bool adapt, float lr, float mom, float wd, float damp,
+                                           float gmul, bool nesterov, bool first) {
+  g = __fmul_rn(g, gmul);
+  if (adapt) g = __fmul_rn(__fmaf_rn(wd, p, g), f);
+  sgd_update(g, p, m, SgdHyper{lr, mom, 0.f, damp, 1.f}, nesterov, first);
+  return make_float2(p, m);
+}
+
+__device__ __forceinline__ void larc_apply(float g, float& p, float& m, const LarcFactor& r, const SgdHyper& h, bool nesterov, bool first) {
+  const float2 pm = larc_update(g, p, m, r.f, r.adapt, h.lr, h.momentum, h.wd, h.dampening, h.gmul, nesterov, first);
+  p = pm.x;
+  m = pm.y;
+}
+
+__device__ __forceinline__ void larc_write_stats(float* stats, int64_t row, const LarcFactor& r) {
+  stats[3 * row] = r.pn;
+  stats[3 * row + 1] = r.gn;
+  stats[3 * row + 2] = r.f;
+}
+
+// Flat front end.  info[t] = {element offset in the flat buffers, numel, first chunk, statistics row}, tensors in
+// ascending offset order; chunk_tensor[q] = tensor of global chunk q.  CTA b runs chunk chunk_lo + b.
+struct LarcChunk { int64_t off, begin, len, cbase, nchunks, row, c; };
+
+__device__ __forceinline__ LarcChunk larc_chunk(const int32_t* chunk_tensor, const int64_t* info, int64_t q) {
+  const int64_t* e = info + 4 * chunk_tensor[q];
+  LarcChunk k;
+  k.off = e[0];
+  k.cbase = e[2];
+  k.row = e[3];
+  k.c = q - k.cbase;
+  k.begin = k.c * kLarcChunk;
+  k.len = min((int64_t)kLarcChunk, e[1] - k.begin);
+  k.nchunks = (e[1] + kLarcChunk - 1) / kLarcChunk;
+  return k;
+}
+
+template <typename G>
+__global__ void __launch_bounds__(kLarcThreads) larc_norm_flat_kernel(const G* __restrict__ grad, const float* __restrict__ master,
+                                                                      const int32_t* __restrict__ chunk_tensor, const int64_t* __restrict__ info,
+                                                                      int64_t chunk_lo, float2* __restrict__ partials,
+                                                                      const float* __restrict__ hyper, const int* __restrict__ found_inf) {
+  if (found_inf && *found_inf) return;
+  const int64_t q = chunk_lo + blockIdx.x;
+  const LarcChunk k = larc_chunk(chunk_tensor, info, q);
+  const G* gp = grad + k.off + k.begin;
+  const float* pp = master + k.off + k.begin;
+  const float gmul = hyper[4];
+  float sp = 0.f, sg = 0.f;
+  for (int64_t i = 8 * threadIdx.x; i < k.len; i += 8 * kLarcThreads) {
+    float p[8], g[8];
+    const int cnt = (int)min((int64_t)8, k.len - i);
+    if (cnt == 8) {
+      load8<G>(gp + i, g, /*sys=*/true);  // arena: bypass L1, as fused_sgd_flat
+      load8<float>(pp + i, p);
+    } else {
+      for (int j = 0; j < cnt; ++j) {
+        g[j] = ldcg_f(gp + i + j);
+        p[j] = pp[i + j];
+      }
+    }
+    larc_acc8(p, g, gmul, cnt, sp, sg);
+  }
+  const float2 s = larc_cta_sum(sp, sg);
+  if (threadIdx.x == 0) partials[q] = s;
+}
+
+template <typename G, typename C, bool HAS_COPY>
+__global__ void __launch_bounds__(kLarcThreads) larc_sgd_flat_kernel(const G* __restrict__ grad, float* __restrict__ master, float* __restrict__ mom,
+                                                                     C* __restrict__ copy, const int32_t* __restrict__ chunk_tensor,
+                                                                     const int64_t* __restrict__ info, int64_t chunk_lo,
+                                                                     const float2* __restrict__ partials, float* __restrict__ stats,
+                                                                     const float* __restrict__ hyper, const int* __restrict__ found_inf,
+                                                                     bool nesterov, bool first, float trust, float eps, bool clip) {
+  if (found_inf && *found_inf) return;  // dynamic loss scaling: skip the step on overflow
+  const SgdHyper h = load_hyper(hyper);
+  first = first || (found_inf && hyper[5] != 0.f);
+  const LarcChunk k = larc_chunk(chunk_tensor, info, chunk_lo + blockIdx.x);
+  const LarcFactor r = larc_factor(partials + k.cbase, k.nchunks, h, trust, eps, clip);
+  if (k.c == 0 && threadIdx.x == 0) larc_write_stats(stats, k.row, r);
+  const int64_t base = k.off + k.begin;
+  for (int64_t i = 8 * threadIdx.x; i < k.len; i += 8 * kLarcThreads) {
+    const int64_t e = base + i;
+    if (k.len - i >= 8) {
+      float g[8], p[8], m[8];
+      load8<G>(grad + e, g, /*sys=*/true);
+      load8<float>(master + e, p);
+      load8<float>(mom + e, m);
+#pragma unroll
+      for (int j = 0; j < 8; ++j) larc_apply(g[j], p[j], m[j], r, h, nesterov, first);
+      store8<float>(master + e, p);
+      store8<float>(mom + e, m);
+      if constexpr (HAS_COPY) store8<C>(copy + e, p);
+    } else {
+      for (int64_t x = e; x < base + k.len; ++x) {
+        float p = master[x], m = mom[x];
+        larc_apply(ldcg_f(grad + x), p, m, r, h, nesterov, first);
+        master[x] = p;
+        mom[x] = m;
+        if constexpr (HAS_COPY) {
+          if constexpr (std::is_same<C, __nv_bfloat16>::value) copy[x] = __float2bfloat16_rn(p);
+          else copy[x] = __float2half_rn(p);
+        }
+      }
+    }
+  }
+}
+
+// Multi-tensor front end: lists 0 grad, 1 fp32 master (norm pass: lists 0 grad, 1 master).
+__global__ void __launch_bounds__(kLarcThreads) larc_norm_multi_kernel(const __grid_constant__ MtaArgs<2> a, const __grid_constant__ LarcSlots s,
+                                                                       float2* __restrict__ partials, const float* __restrict__ hyper,
+                                                                       const int* __restrict__ found_inf) {
+  if (found_inf && *found_inf) return;
+  const int t = a.block_tensor[blockIdx.x];
+  const int c = a.block_chunk[blockIdx.x];
+  const int64_t begin = (int64_t)c * kLarcChunk;
+  const int64_t len = min((int64_t)kLarcChunk, a.numel[t] - begin);
+  const float* pp = reinterpret_cast<const float*>(a.ptr[1][t]) + begin;
+  const int gdt = a.dtype[0][t];
+  const float gmul = hyper[4];
+  float sp = 0.f, sg = 0.f;
+  for (int64_t i = 8 * threadIdx.x; i < len; i += 8 * kLarcThreads) {
+    float p[8], g[8];
+    const int cnt = (int)min((int64_t)8, len - i);
+    for (int j = 0; j < cnt; ++j) {
+      g[j] = ld_any(a.ptr[0][t], gdt, begin + i + j);
+      p[j] = pp[i + j];
+    }
+    larc_acc8(p, g, gmul, cnt, sp, sg);
+  }
+  const float2 r = larc_cta_sum(sp, sg);
+  if (threadIdx.x == 0) partials[s.cbase[t] + c] = r;
+}
+
+// lists: 0 grad, 1 fp32 master, 2 momentum (fp32), 3 model copy (optional: ptr may be null)
+__global__ void __launch_bounds__(kLarcThreads) larc_sgd_multi_kernel(const __grid_constant__ MtaArgs<4> a, const __grid_constant__ LarcSlots s,
+                                                                      const float2* __restrict__ partials, float* __restrict__ stats,
+                                                                      const float* __restrict__ hyper, const int* __restrict__ found_inf,
+                                                                      bool nesterov, float trust, float eps, bool clip) {
+  if (found_inf && *found_inf) return;
+  const SgdHyper h = load_hyper(hyper);
+  const int t = a.block_tensor[blockIdx.x];
+  const bool first = s.first[t] || (found_inf && hyper[5] != 0.f);
+  const int c = a.block_chunk[blockIdx.x];
+  const LarcFactor r = larc_factor(partials + s.cbase[t], (a.numel[t] + kLarcChunk - 1) / kLarcChunk, h, trust, eps, clip);
+  if (c == 0 && threadIdx.x == 0) larc_write_stats(stats, s.row[t], r);
+  const int64_t begin = (int64_t)c * kLarcChunk;
+  const int64_t end = min(begin + (int64_t)kLarcChunk, a.numel[t]);
+  float* p = reinterpret_cast<float*>(a.ptr[1][t]);
+  float* m = reinterpret_cast<float*>(a.ptr[2][t]);
+  const int gdt = a.dtype[0][t], cdt = a.dtype[3][t];
+  for (int64_t i = begin + threadIdx.x; i < end; i += blockDim.x) {
+    float pv = p[i], mv = m[i];
+    larc_apply(ld_any(a.ptr[0][t], gdt, i), pv, mv, r, h, nesterov, first);
+    p[i] = pv;
+    m[i] = mv;
+    if (a.ptr[3][t]) st_any(a.ptr[3][t], cdt, i, pv);
+  }
+}
+
+static void check_larc_common(const at::Tensor& hyper, const c10::optional<at::Tensor>& found_inf, const at::Tensor& stats, double trust,
+                              double eps) {
+  TORCH_CHECK(hyper.scalar_type() == at::kFloat && hyper.numel() >= 5, "hyper must be fp32 with slots 0..4");
+  TORCH_CHECK(!found_inf.has_value() || hyper.numel() >= 6, "hyper needs slot 5 (momentum_pending) when found_inf is given");
+  TORCH_CHECK(stats.scalar_type() == at::kFloat && stats.is_contiguous(), "LARC statistics must be a contiguous fp32 tensor");
+  TORCH_CHECK(std::isfinite(trust) && trust > 0 && std::isfinite(eps) && eps >= 0, "LARC needs trust_coefficient > 0 and eps >= 0");
+}
+
+// calls fn(G{}, C{}, has_copy) with the gradient / model-copy types of fused_sgd_flat's instantiations
+template <typename Fn>
+static void larc_flat_types(at::ScalarType gt, c10::optional<at::ScalarType> ct, Fn&& fn) {
+  auto with_copy = [&](auto g) {
+    if (!ct.has_value()) fn(g, float{}, std::false_type{});
+    else if (*ct == at::kBFloat16) fn(g, __nv_bfloat16{}, std::true_type{});
+    else if (*ct == at::kHalf) fn(g, __half{}, std::true_type{});
+    else TORCH_CHECK(false, "unsupported model copy dtype");
+  };
+  if (gt == at::kBFloat16) with_copy(__nv_bfloat16{});
+  else if (gt == at::kHalf) with_copy(__half{});
+  else if (gt == at::kFloat) with_copy(float{});
+  else TORCH_CHECK(false, "unsupported gradient dtype");
+}
+
+void larc_sgd_flat(at::Tensor grad, at::Tensor master, at::Tensor momentum, c10::optional<at::Tensor> model_copy, at::Tensor hyper,
+                   c10::optional<at::Tensor> found_inf, bool nesterov, bool first_step, at::Tensor chunk_tensor, at::Tensor info,
+                   int64_t chunk_lo, int64_t chunk_hi, at::Tensor partials, at::Tensor stats, double trust, double eps, bool clip) {
+  const int64_t n = master.numel();
+  TORCH_CHECK(grad.numel() >= n && momentum.numel() == n, "flat buffer size mismatch");
+  TORCH_CHECK(master.scalar_type() == at::kFloat && momentum.scalar_type() == at::kFloat);
+  TORCH_CHECK(master.is_contiguous() && momentum.is_contiguous() && grad.is_contiguous());
+  check_larc_common(hyper, found_inf, stats, trust, eps);
+  TORCH_CHECK(chunk_tensor.scalar_type() == at::kInt && info.scalar_type() == at::kLong && info.dim() == 2 && info.size(1) == 4 &&
+                  chunk_tensor.is_contiguous() && info.is_contiguous(), "LARC chunk table: int32 [chunks] and int64 [tensors, 4]");
+  TORCH_CHECK(0 <= chunk_lo && chunk_lo <= chunk_hi && chunk_hi <= chunk_tensor.numel(), "LARC chunk range outside the table");
+  TORCH_CHECK(partials.scalar_type() == at::kFloat && partials.is_contiguous() && partials.numel() >= 2 * chunk_tensor.numel(),
+              "LARC partials: fp32 [2 * chunks]");
+  if (model_copy.has_value()) TORCH_CHECK(model_copy->numel() == n && model_copy->is_contiguous());
+  if (chunk_hi == chunk_lo) return;
+  c10::cuda::CUDAGuard guard(master.device());
+  cudaStream_t st = at::cuda::getCurrentCUDAStream();
+  const int* fi = found_inf.has_value() ? reinterpret_cast<const int*>(found_inf->data_ptr()) : nullptr;
+  const int grid = (int)(chunk_hi - chunk_lo);
+  const int32_t* ct = chunk_tensor.data_ptr<int32_t>();
+  const int64_t* inf = info.data_ptr<int64_t>();
+  float2* part = reinterpret_cast<float2*>(partials.data_ptr<float>());
+  const float* hp = hyper.data_ptr<float>();
+  larc_flat_types(grad.scalar_type(), model_copy.has_value() ? c10::optional<at::ScalarType>(model_copy->scalar_type()) : c10::nullopt,
+                  [&](auto g, auto c, auto has_copy) {
+                    using G = decltype(g);
+                    using C = decltype(c);
+                    const G* gp = reinterpret_cast<const G*>(grad.data_ptr());
+                    larc_norm_flat_kernel<G><<<grid, kLarcThreads, 0, st>>>(gp, master.data_ptr<float>(), ct, inf, chunk_lo, part, hp, fi);
+                    C10_CUDA_KERNEL_LAUNCH_CHECK();
+                    C* cp = has_copy ? reinterpret_cast<C*>(model_copy->data_ptr()) : nullptr;
+                    larc_sgd_flat_kernel<G, C, decltype(has_copy)::value><<<grid, kLarcThreads, 0, st>>>(
+                        gp, master.data_ptr<float>(), momentum.data_ptr<float>(), cp, ct, inf, chunk_lo, part, stats.data_ptr<float>(), hp, fi,
+                        nesterov, first_step, (float)trust, (float)eps, clip);
+                    C10_CUDA_KERNEL_LAUNCH_CHECK();
+                  });
+}
+
+void larc_sgd_multi(std::vector<at::Tensor> grads, std::vector<at::Tensor> params, std::vector<at::Tensor> momenta,
+                    std::vector<c10::optional<at::Tensor>> model_copies, at::Tensor hyper, c10::optional<at::Tensor> found_inf, bool nesterov,
+                    std::vector<bool> first, std::vector<int64_t> rows, at::Tensor stats, double trust, double eps, bool clip) {
+  const size_t n = params.size();
+  if (n == 0) return;
+  TORCH_CHECK(grads.size() == n && momenta.size() == n && first.size() == n && rows.size() == n, "LARC lists must have one entry per tensor");
+  TORCH_CHECK(model_copies.empty() || model_copies.size() == n);
+  for (auto& p : params) TORCH_CHECK(p.scalar_type() == at::kFloat, "params (masters) must be fp32");
+  for (auto& m : momenta) TORCH_CHECK(m.scalar_type() == at::kFloat, "momentum must be fp32");
+  check_larc_common(hyper, found_inf, stats, trust, eps);
+  std::vector<at::Tensor> copies;
+  for (auto& c : model_copies) copies.push_back(c.has_value() ? *c : at::Tensor());
+  std::vector<int32_t> cbase(n);
+  int64_t chunks = 0;
+  for (size_t i = 0; i < n; ++i) {
+    TORCH_CHECK(rows[i] >= 0 && 3 * (rows[i] + 1) <= stats.numel(), "LARC statistics row outside the buffer");
+    cbase[i] = (int32_t)chunks;
+    chunks += (params[i].numel() + kLarcChunk - 1) / kLarcChunk;
+  }
+  TORCH_CHECK(chunks < INT32_MAX, "too many LARC chunks");
+  c10::cuda::CUDAGuard guard(params[0].device());
+  cudaStream_t st = at::cuda::getCurrentCUDAStream();
+  const int* fi = found_inf.has_value() ? reinterpret_cast<const int*>(found_inf->data_ptr()) : nullptr;
+  const float* hp = hyper.data_ptr<float>();
+  at::Tensor partials = at::empty({std::max<int64_t>(2 * chunks, 2)}, params[0].options());
+  float2* part = reinterpret_cast<float2*>(partials.data_ptr<float>());
+  auto slots = [&](const int* src, int count) {
+    LarcSlots s{};
+    for (int k = 0; k < count; ++k) {
+      s.cbase[k] = cbase[src[k]];
+      s.row[k] = (int32_t)rows[src[k]];
+      s.first[k] = first[src[k]] ? 1 : 0;
+    }
+    return s;
+  };
+  // every norm of the list is formed before any update launch
+  mta_for_each<2>({grads, params}, [&](const MtaArgs<2>& a, int nb, const int* src) {
+    larc_norm_multi_kernel<<<nb, kLarcThreads, 0, st>>>(a, slots(src, a.block_tensor[nb - 1] + 1), part, hp, fi);
+    C10_CUDA_KERNEL_LAUNCH_CHECK();
+  });
+  mta_for_each<4>({grads, params, momenta, copies}, [&](const MtaArgs<4>& a, int nb, const int* src) {
+    larc_sgd_multi_kernel<<<nb, kLarcThreads, 0, st>>>(a, slots(src, a.block_tensor[nb - 1] + 1), part, stats.data_ptr<float>(), hp, fi,
+                                                       nesterov, (float)trust, (float)eps, clip);
     C10_CUDA_KERNEL_LAUNCH_CHECK();
   });
 }

@@ -335,9 +335,14 @@ class Strategy:
     def make_optimizer(self, model, args):
         if args.optimizer == "fused":
             from .ops.fused_sgd import FusedSGD
-            return FusedSGD(model.parameters(), args.lr, momentum=args.momentum, weight_decay=args.weight_decay,
-                            overlap_backward=bool(getattr(args, "overlap_optimizer", False)) and self.overlap_optimizer)
-        return torch.optim.SGD(model.parameters(), args.lr, momentum=args.momentum, weight_decay=args.weight_decay)
+            opt = FusedSGD(model.parameters(), args.lr, momentum=args.momentum, weight_decay=args.weight_decay,
+                           overlap_backward=bool(getattr(args, "overlap_optimizer", False)) and self.overlap_optimizer)
+        else:
+            opt = torch.optim.SGD(model.parameters(), args.lr, momentum=args.momentum, weight_decay=args.weight_decay)
+        if getattr(args, "larc", False):
+            from .apex.parallel.LARC import LARC
+            opt = LARC(opt, trust_coefficient=args.larc_trust_coefficient, clip=args.larc_clip)
+        return opt
 
     def wrap(self, model, args, device, local_rank):
         from .parallel.ddp import DistributedDataParallel

@@ -9,6 +9,9 @@ Three execution modes, picked automatically:
     flat buffers with the arena's layout, and the whole step is ONE streaming kernel.
   * **multi-tensor** - CUDA parameters without an engine: chunked multi-tensor-apply kernel over ``p.grad``.
   * **reference** - CPU tensors: plain PyTorch math (also the numerical oracle for the tests).
+
+``enable_larc`` (what ``apex.parallel.LARC`` calls) adds layer-wise adaptive rates to all three modes: a norm pass and an
+update pass per flat step, per bucket in overlap mode, or per group in multi-tensor mode (``csrc/optim.cu``).
 """
 from __future__ import annotations
 
@@ -16,6 +19,9 @@ from typing import Optional
 
 import torch
 from torch.optim import Optimizer
+
+
+_FP32_STATE = ("momentum_buffer", "master")     # per-parameter state that stays fp32 whatever the parameter's dtype
 
 
 def sgd_reference_step(p, g, buf, lr, momentum, weight_decay, dampening, nesterov, first):
@@ -30,6 +36,19 @@ def sgd_reference_step(p, g, buf, lr, momentum, weight_decay, dampening, nestero
             buf.mul_(momentum).add_(g, alpha=1 - dampening)
         g = g.add(buf, alpha=momentum) if nesterov else buf
     p.add_(g.to(p.dtype), alpha=-lr)
+
+
+def larc_reference_grad(p, g, lr, weight_decay, trust_coefficient, clip, eps):
+    """apex.parallel.LARC on one tensor in fp32: the gradient the wrapped SGD step (run with weight_decay = 0) sees, and
+    ``(pn, gn, f)``.  Where a norm is zero the gradient is left as is, without weight decay, and f is reported as 1."""
+    p, g = p.float(), g.float()
+    pn, gn = torch.linalg.vector_norm(p), torch.linalg.vector_norm(g)
+    if pn == 0 or gn == 0:
+        return g, (float(pn), float(gn), 1.0)
+    f = trust_coefficient * pn / (gn + pn * weight_decay + eps)
+    if clip:
+        f = torch.clamp(f / lr, max=1.0)
+    return (g + weight_decay * p) * f, (float(pn), float(gn), float(f))
 
 
 class FusedSGD(Optimizer):
@@ -54,6 +73,9 @@ class FusedSGD(Optimizer):
         self._ov_applied = 0
         self._ov_first = False
         self._bind_refused = False  # an engine was found but declined (mixed dtypes, other parameter list): do not retry
+        self._larc = None           # (trust_coefficient, clip, eps) in LARC mode (enable_larc)
+        self._larc_stats = None     # [n_params, 3] fp32 {pn, gn, f} of the last applied step
+        self._larc_tab = None       # flat mode: chunk table of the arena layout (built once)
         self._try_bind()
 
     # ------------------------------------------------------------------ engine binding (flat mode)
@@ -97,11 +119,88 @@ class FusedSGD(Optimizer):
             return
         fs = self._flat
         from .. import _ext
+        if self._larc is not None:
+            self._larc_flat(self._hyper[0][0], None, self._ov_first, self._larc_table().ranges[(off, n)])
+            self._ov_applied += n
+            return
         _ext.note_launch()
         copy = fs.model_copy[off:off + n] if fs.model_copy is not None else None
         _ext.lib().fused_sgd_flat(fs.engine.grad_arena()[off:off + n], fs.master[off:off + n], fs.momentum[off:off + n], copy,
                                   self._hyper[0][0], None, bool(self.param_groups[0]["nesterov"]), self._ov_first)
         self._ov_applied += n
+
+    # ------------------------------------------------------------------ LARC (apex.parallel.LARC semantics)
+    def enable_larc(self, trust_coefficient: float = 0.02, clip: bool = True, eps: float = 1e-8) -> None:
+        """Layer-wise adaptive rates on top of every step (what wrapping this optimizer in ``apex.parallel.LARC`` does)."""
+        if not (trust_coefficient > 0 and eps >= 0):
+            raise ValueError("LARC needs trust_coefficient > 0 and eps >= 0")
+        self._larc = (float(trust_coefficient), bool(clip), float(eps))
+
+    def larc_stats(self) -> Optional[torch.Tensor]:
+        """``[n_params, 3]`` fp32 ``(||p||, ||g||, f)`` per parameter in ``param_groups`` order, as of the last applied LARC step
+        (f = 1 where a norm is zero; rows of parameters without a gradient stay as they were).  None before the first one."""
+        return self._larc_stats
+
+    def _larc_rows(self):
+        return {id(p): i for i, p in enumerate(p for g in self.param_groups for p in g["params"])}
+
+    def _larc_stats_on(self, device):
+        n = sum(len(g["params"]) for g in self.param_groups)
+        old = self._larc_stats
+        if old is None or old.size(0) != n:
+            # first LARC step, or add_param_group since: rows keep param_groups order, the existing ones keep their values
+            self._larc_stats = torch.zeros(n, 3, dtype=torch.float32, device=device)
+            if old is not None:
+                k = min(n, old.size(0))
+                self._larc_stats[:k].copy_(old[:k])
+        return self._larc_stats
+
+    def _larc_table(self):
+        """Chunk table of the flat layout: tensors in arena order with their first chunk, and the chunk range of every
+        gradient bucket.  The layout never changes after binding, so this is built once and kept on the device."""
+        if self._larc_tab is not None:
+            return self._larc_tab
+        from types import SimpleNamespace
+        from .. import _ext
+        chunk = _ext.lib().LARC_CHUNK
+        eng = self._flat.engine
+        rows = self._larc_rows()
+        order = sorted(range(len(eng.params)), key=lambda i: eng.param_elem_off[i])
+        info, chunk_tensor, spans = [], [], []
+        for t, pid in enumerate(order):
+            p, off = eng.params[pid], eng.param_elem_off[pid]
+            assert not spans or off >= spans[-1][1], "flat LARC: parameters overlap in the arena"
+            info.append((off, p.numel(), len(chunk_tensor), rows[id(p)]))
+            spans.append((off, off + p.numel(), len(chunk_tensor)))
+            chunk_tensor += [t] * (-(-p.numel() // chunk))
+        assert not spans or spans[-1][1] <= self._flat.master.numel()
+        ranges = {}
+        for b in getattr(eng, "buckets", []):
+            lo, hi = b.elem_off, b.elem_off + b.region_elems
+            inside = [s for s in spans if lo <= s[0] < hi]
+            # buckets hold whole tensors (plan.compute_buckets): a tensor's norm never spans two per-bucket launches
+            assert all(s[1] <= hi for s in inside), "flat LARC: a gradient bucket splits a tensor"
+            first = inside[0][2] if inside else 0
+            last = inside[-1][2] + -(-(inside[-1][1] - inside[-1][0]) // chunk) if inside else 0
+            ranges[(b.elem_off, b.region_elems)] = (first, last)
+        dev = self._flat.master.device
+        self._larc_tab = SimpleNamespace(
+            chunk_tensor=torch.tensor(chunk_tensor, dtype=torch.int32, device=dev),
+            info=torch.tensor(info, dtype=torch.int64, device=dev).reshape(-1, 4),
+            partials=torch.zeros(max(2 * len(chunk_tensor), 2), dtype=torch.float32, device=dev),
+            chunks=len(chunk_tensor), ranges=ranges)
+        return self._larc_tab
+
+    def _larc_flat(self, hyper, found_inf, first, chunk_range=None):
+        fs = self._flat
+        tab = self._larc_table()
+        lo, hi = chunk_range if chunk_range is not None else (0, tab.chunks)
+        trust, clip, eps = self._larc
+        from .. import _ext
+        _ext.note_launch(2)
+        _ext.lib().larc_sgd_flat(fs.engine.grad_arena(), fs.master, fs.momentum, fs.model_copy, hyper, found_inf,
+                                 bool(self.param_groups[0]["nesterov"]), first, tab.chunk_tensor, tab.info, lo, hi, tab.partials,
+                                 self._larc_stats_on(fs.master.device), trust, eps, clip)
 
     @property
     def is_flat(self) -> bool:
@@ -158,9 +257,12 @@ class FusedSGD(Optimizer):
             if amp is not None:
                 amp.attach_hyper(hyper)
             from .. import _ext
-            _ext.note_launch()
-            _ext.lib().fused_sgd_flat(fs.engine.grad_arena(), fs.master, fs.momentum, fs.model_copy, hyper,
-                                      amp.found_inf if amp is not None else None, bool(group["nesterov"]), first)
+            if self._larc is not None:
+                self._larc_flat(hyper, amp.found_inf if amp is not None else None, first)
+            else:
+                _ext.note_launch()
+                _ext.lib().fused_sgd_flat(fs.engine.grad_arena(), fs.master, fs.momentum, fs.model_copy, hyper,
+                                          amp.found_inf if amp is not None else None, bool(group["nesterov"]), first)
             if amp is not None:
                 amp.update()
         else:
@@ -201,6 +303,19 @@ class FusedSGD(Optimizer):
                         del p._ptd_master_init
                 return st["master"]
 
+            if self._larc is not None:
+                # one call: every norm of the group is formed before any update; `fresh` travels as a per-tensor first flag
+                rows = self._larc_rows()
+                trust, clip, eps = self._larc
+                fresh_ids = {id(p) for p in fresh}
+                _ext.note_launch(2)
+                C.larc_sgd_multi([p.grad for p in params], [p if p.dtype == torch.float32 else master_of(p) for p in params],
+                                 [self.state[p]["momentum_buffer"] for p in params],
+                                 [None if p.dtype == torch.float32 else p.data for p in params], hyper,
+                                 amp.found_inf if amp is not None else None, bool(group["nesterov"]),
+                                 [id(p) in fresh_ids for p in params], [rows[id(p)] for p in params],
+                                 self._larc_stats_on(params[0].device), trust, eps, clip)
+                return
             fs = set(fresh) if (fresh and len(fresh) != len(params)) else None      # rare: first gradient later than the others
             for first_flag, sub in ((True, fresh), (False, [p for p in params if p not in fs])) if fs is not None else ((bool(fresh), params),):
                 full = [p for p in sub if p.dtype == torch.float32]
@@ -216,19 +331,23 @@ class FusedSGD(Optimizer):
             if amp is not None and amp.host_found_inf():
                 return
             gmul = amp.host_inv_scale() if amp is not None else 1.0
+            rows = self._larc_rows() if self._larc is not None else None
             for p, buf in zip(params, bufs):
                 fresh = self.state[p].pop("_fresh", False)
                 g = p.grad if gmul == 1.0 else p.grad.float() * gmul
-                if p.dtype == torch.float32:
-                    sgd_reference_step(p, g, buf, group["lr"], group["momentum"], group["weight_decay"], group["dampening"],
-                                       group["nesterov"], fresh)
-                else:
-                    st = self.state[p]
-                    if "master" not in st:
-                        st["master"] = p.detach().float().clone()
-                    sgd_reference_step(st["master"], g, buf, group["lr"], group["momentum"], group["weight_decay"],
-                                       group["dampening"], group["nesterov"], fresh)
-                    p.copy_(st["master"])
+                st = self.state[p]
+                if p.dtype != torch.float32 and "master" not in st:
+                    st["master"] = p.detach().float().clone()
+                master = p if p.dtype == torch.float32 else st["master"]
+                wd = group["weight_decay"]
+                if rows is not None:
+                    trust, clip, eps = self._larc
+                    g, stats = larc_reference_grad(master, g, group["lr"], wd, trust, clip, eps)
+                    self._larc_stats_on(p.device)[rows[id(p)]] = torch.tensor(stats)
+                    wd = 0.0
+                sgd_reference_step(master, g, buf, group["lr"], group["momentum"], wd, group["dampening"], group["nesterov"], fresh)
+                if master is not p:
+                    p.copy_(master)
 
     def zero_grad(self, set_to_none: bool = True):
         super().zero_grad(set_to_none=set_to_none)
@@ -236,7 +355,17 @@ class FusedSGD(Optimizer):
     def load_state_dict(self, state_dict):
         """Standard ``Optimizer.load_state_dict``; in flat mode the loaded momentum is copied INTO the flat buffer
         (the kernel reads that buffer, not the per-parameter tensors) and the state entries are re-pointed at its views."""
+        # torch casts loaded state to the parameter's dtype, but momentum and masters are fp32 whatever the model copy is (the
+        # kernels require it): put the saved fp32 values back, for every order of binding (bound now, bound later through
+        # bind_flat_optimizer, or never: multi-tensor / CPU)
+        saved_ids = [i for g in state_dict["param_groups"] for i in g["params"]]
+        own = [p for g in self.param_groups for p in g["params"]]
+        saved = {id(p): {k: v for k, v in state_dict["state"].get(i, {}).items() if k in _FP32_STATE and torch.is_tensor(v)}
+                 for p, i in zip(own, saved_ids)}
         super().load_state_dict(state_dict)
+        for p in own:
+            for k, v in saved[id(p)].items():
+                self.state[p][k] = v.to(device=p.device, dtype=torch.float32)
         loaded = False
         if self._flat is not None:
             eng = self._flat.engine

@@ -24,6 +24,12 @@ KERNELS = [
     (r"fused_sgd_flat_kernelI13__nv_bfloat16S1_Lb1E", "fused_sgd_flat_kernel<bf16 grad, bf16 model>", "optim.cu",
      "K6: unscale + overflow skip + SGD momentum over arena / fp32 masters / momentum / bf16 copy", "tests/test_gpu_kernels.py"),
     (r"fused_sgd_multi_kernel", "fused_sgd_multi_kernel", "optim.cu", "multi-tensor-apply variant (non-flat parameters)", "tests/test_gpu_kernels.py"),
+    (r"larc_norm_flat_kernelI13__nv_bfloat16E", "larc_norm_flat_kernel<bf16>", "optim.cu",
+     "LARC norm pass: per-chunk fp32 sums of p^2 and (g gmul)^2 over the arena, fixed order", "tests/test_gpu_larc.py, tools/larc_bench.py"),
+    (r"larc_sgd_flat_kernelI13__nv_bfloat16S1_Lb1E", "larc_sgd_flat_kernel<bf16 grad, bf16 model>", "optim.cu",
+     "LARC update: trust ratio from the chunk partials + SGD momentum + bf16 copy + statistics", "tests/test_gpu_larc.py, tools/larc_bench.py"),
+    (r"larc_norm_multi_kernel", "larc_norm_multi_kernel", "optim.cu", "LARC norm pass, multi-tensor-apply variant", "tests/test_gpu_larc.py"),
+    (r"larc_sgd_multi_kernel", "larc_sgd_multi_kernel", "optim.cu", "LARC update, multi-tensor-apply variant", "tests/test_gpu_larc.py"),
     (r"multi_tensor_scale_kernel", "multi_tensor_scale_kernel", "optim.cu", "amp unscale with non-finite flag", "tests/test_gpu_kernels.py"),
     (r"amp_update_scale_kernel", "amp_update_scale_kernel", "optim.cu", "loss-scale state machine on the device", "tests/test_gpu_kernels.py"),
     (r"bn_stats_kernelI13__nv_bfloat16E", "bn_stats_kernel<bf16>", "bn_act.cu", "BN forward statistics (one row of partial sums per CTA)", "tests/test_gpu_kernels.py"),
