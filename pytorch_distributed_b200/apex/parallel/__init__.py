@@ -8,6 +8,8 @@ dynamic loss scaling is on - the non-finite test folded into the all-reduce so a
 """
 from __future__ import annotations
 
+from contextlib import contextmanager
+
 import torch
 import torch.nn as nn
 
@@ -34,12 +36,16 @@ class DistributedDataParallel(nn.Module):
     ``retain_allreduce_buffers``  ``self.allreduce_buffers`` = the per-bucket flat slices of the symmetric gradient arena
     ``num_allreduce_streams`` > 1, ``allreduce_communicators``, ``allreduce_trigger_params``, ``shared_param`` are rejected:
     there is one communication stream and one (symmetric-memory) communicator by design.
+
+    Extensions (apex has neither): ``no_sync()``, torch DDP's context for backwards that only accumulate, and
+    ``fp32_grad_accumulation``, which keeps that running sum in fp32 outside ``p.grad`` (see ``GradientEngine``).
     """
 
     def __init__(self, module: nn.Module, message_size: int = 10000000, delay_allreduce: bool = False, shared_param=None,
                  allreduce_trigger_params=None, retain_allreduce_buffers: bool = False, allreduce_always_fp32: bool = False,
                  num_allreduce_streams: int = 1, allreduce_communicators=None, gradient_average: bool = True,
-                 gradient_predivide_factor: float = 1.0, comm="auto", wire_dtype=None, process_group=None):
+                 gradient_predivide_factor: float = 1.0, comm="auto", wire_dtype=None, process_group=None,
+                 fp32_grad_accumulation: bool = False):
         super().__init__()
         if shared_param is not None:
             raise ValueError("shared_param is no longer supported as an option (apex removed it as well); use delay_allreduce=True")
@@ -74,7 +80,8 @@ class DistributedDataParallel(nn.Module):
         scale = (1.0 / world) if gradient_average else (1.0 / float(gradient_predivide_factor))
         self.engine = GradientEngine(params, comm, wire_dtype=wire_dtype, bucket_cap_mb=message_size * esz / float(1 << 20),
                                      first_bucket_mb=message_size * esz / float(1 << 20), check_inf=check_inf,
-                                     average=gradient_average, delay_allreduce=delay_allreduce, scale=scale, tail_bucket_mb=None)
+                                     average=gradient_average, delay_allreduce=delay_allreduce, scale=scale, tail_bucket_mb=None,
+                                     fp32_grad_accumulation=fp32_grad_accumulation)
         self.delay_allreduce = delay_allreduce
         self.gradient_average = gradient_average
         self.gradient_predivide_factor = gradient_predivide_factor
@@ -92,6 +99,16 @@ class DistributedDataParallel(nn.Module):
 
     def forward(self, *inputs, **kwargs):
         return self.module(*inputs, **kwargs)
+
+    @contextmanager
+    def no_sync(self):
+        """Backwards inside this context reduce nothing across ranks (torch DDP's ``no_sync``; an extension here)."""
+        old = self.engine.enabled
+        self.engine.enabled = False
+        try:
+            yield
+        finally:
+            self.engine.enabled = old
 
 
 class Reducer:

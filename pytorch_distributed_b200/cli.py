@@ -97,6 +97,9 @@ def build_parser(entry: str = "distributed") -> argparse.ArgumentParser:
                    help="LARC clip mode: the adaptive factor is min(f / lr, 1) (default)")
     x.add_argument("--no-larc-clip", dest="larc_clip", action="store_false",
                    help="LARC scale mode: the gradient is multiplied by f itself")
+    x.add_argument("--accum-steps", default=1, type=_positive_int, metavar="N",
+                   help="gradient accumulation: one optimizer step per N consecutive batches (effective batch -b x N); the fused "
+                        "engine sums the earlier passes in fp32 on each GPU and reduces once, in the last pass (default: 1)")
     x.add_argument("--cuda-graph", action="store_true", help="capture the train step in a CUDA graph")
     x.add_argument("--sync-bn", action="store_true",
                    help="synchronise BatchNorm statistics across the data-parallel ranks (torch.nn.SyncBatchNorm semantics; "
@@ -125,6 +128,13 @@ def resolve_local_rank(args) -> int:
     return lr
 
 
+def _positive_int(s: str) -> int:
+    v = int(s)
+    if v < 1:
+        raise argparse.ArgumentTypeError("must be an integer >= 1, got %r" % (s,))
+    return v
+
+
 def _positive_float(s: str) -> float:
     v = float(s)
     if not (v > 0 and math.isfinite(v)):
@@ -137,6 +147,11 @@ def parse_args(entry: str, argv=None):
     args = parser.parse_args(argv)
     if not args.larc and (args.larc_trust_coefficient is not None or args.larc_clip is not None):
         parser.error("--larc-trust-coefficient / --larc-clip / --no-larc-clip need --larc")
+    if args.accum_steps > 1 and entry == "dataparallel":
+        parser.error("--accum-steps needs one process per GPU; the single-process DataParallel entrypoint does not support it")
+    if args.steps_per_epoch is not None and args.steps_per_epoch < args.accum_steps:
+        parser.error("--steps-per-epoch %d is less than --accum-steps %d: an epoch would hold no optimizer step" %
+                     (args.steps_per_epoch, args.accum_steps))
     if args.larc_trust_coefficient is None:
         args.larc_trust_coefficient = 0.02
     if args.larc_clip is None:

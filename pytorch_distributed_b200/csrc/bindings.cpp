@@ -105,6 +105,16 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
            py::arg("channel"), py::arg("xoff"), py::arg("calls_ptr"), py::arg("as_rank") = 0);
 
   m.def("pack_pointers", &pack_pointers);
+  m.def("grad_accumulate",
+        [](const std::vector<at::Tensor>& grads, const at::Tensor& seg_begin, const at::Tensor& segs, int64_t grid, int64_t split, at::Tensor acc,
+           int64_t acc_off, int64_t region_elems) { grad_accum(grads, seg_begin, segs, grid, split, acc, acc_off, region_elems, false); },
+        py::arg("grads"), py::arg("seg_begin"), py::arg("segs"), py::arg("grid"), py::arg("split"), py::arg("acc"), py::arg("acc_off"),
+        py::arg("region_elems"));
+  m.def("grad_fold",
+        [](const std::vector<at::Tensor>& grads, const at::Tensor& seg_begin, const at::Tensor& segs, int64_t grid, int64_t split, at::Tensor acc,
+           int64_t acc_off, int64_t region_elems) { grad_accum(grads, seg_begin, segs, grid, split, acc, acc_off, region_elems, true); },
+        py::arg("grads"), py::arg("seg_begin"), py::arg("segs"), py::arg("grid"), py::arg("split"), py::arg("acc"), py::arg("acc_off"),
+        py::arg("region_elems"));
   m.def("fused_sgd_flat", &fused_sgd_flat, py::arg("grad"), py::arg("master"), py::arg("momentum"), py::arg("model_copy"), py::arg("hyper"),
         py::arg("found_inf"), py::arg("nesterov"), py::arg("first_step"));
   m.def("fused_sgd_multi", &fused_sgd_multi);

@@ -595,6 +595,97 @@ __global__ void ll_allreduce_kernel(const __grid_constant__ CommCtx c, const flo
   if (lane == 0) *ll_seq = seq;
 }
 
+// ================================================================= rank-local fp32 gradient accumulation (no peers)
+// Driven by a bucket's plan (segment table + pointer pack), one launch per bucket and pass, nothing crosses GPUs.  `acc`
+// is the bucket's slice of an fp32 buffer with the gradient arena's element layout (element acc[seg.arena_off + i]).
+//   grad_accumulate : acc += float(g)                                   (every pass of a no_sync group but the last)
+//   grad_fold       : g = round_to_dtype(acc + float(g)); acc = 0       (the last pass, right before K1)
+// Each element is one IEEE fp32 add in pass order (add.rn.f32: no contraction, denormals kept), so the sum is the one
+// torch's acc.add_(g.float()) / (acc + g.float()).to(g.dtype) give.  Only the segments' elements are touched: the padding
+// between tensors is never written.  blockIdx.y splits every plan CTA's segments over gridDim.y CTAs.
+__device__ __forceinline__ float add_rn(float a, float b) {
+  float r;
+  asm("add.rn.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b));
+  return r;
+}
+
+template <bool kFold, typename S>
+__device__ __forceinline__ void accum_seg(S* __restrict__ g, float* __restrict__ acc, int len) {
+  const int stride = blockDim.x * gridDim.y;
+  const int t0 = threadIdx.x + blockIdx.y * blockDim.x;
+  // acc is 32-byte aligned at every segment start (arena offsets are multiples of 8 elements); the gradient may not be
+  const bool aligned = ((reinterpret_cast<uintptr_t>(g) & 15) == 0);
+  const int nvec = aligned ? (len >> 3) : 0;
+  int v = t0;
+  for (; v + stride < nvec; v += 2 * stride) {       // two independent 8-element units in flight per thread
+    float f[2][8], a[2][8];
+#pragma unroll
+    for (int u = 0; u < 2; ++u) {
+      load8<S>(g + ((v + u * stride) << 3), f[u]);
+      load8<float>(acc + ((v + u * stride) << 3), a[u]);
+    }
+#pragma unroll
+    for (int u = 0; u < 2; ++u) {
+#pragma unroll
+      for (int k = 0; k < 8; ++k) a[u][k] = add_rn(a[u][k], f[u][k]);
+      if constexpr (kFold) {
+        store8<S>(g + ((v + u * stride) << 3), a[u]);
+        const float z[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+        store8<float>(acc + ((v + u * stride) << 3), z);
+      } else {
+        store8<float>(acc + ((v + u * stride) << 3), a[u]);
+      }
+    }
+  }
+  for (; v < nvec; v += stride) {
+    float f[8], a[8];
+    load8<S>(g + (v << 3), f);
+    load8<float>(acc + (v << 3), a);
+#pragma unroll
+    for (int k = 0; k < 8; ++k) a[k] = add_rn(a[k], f[k]);
+    if constexpr (kFold) {
+      store8<S>(g + (v << 3), a);
+      const float z[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+      store8<float>(acc + (v << 3), z);
+    } else {
+      store8<float>(acc + (v << 3), a);
+    }
+  }
+  for (int i = (nvec << 3) + t0; i < len; i += stride) {
+    const float s = add_rn(acc[i], to_f32<S>(g[i]));
+    if constexpr (kFold) {
+      g[i] = from_f32<S>(s);
+      acc[i] = 0.f;
+    } else {
+      acc[i] = s;
+    }
+  }
+}
+
+template <bool kFold>
+__device__ __forceinline__ void accum_block(const PtrPack& pk, const int32_t* __restrict__ seg_begin, const Seg* __restrict__ segs,
+                                            float* __restrict__ acc) {
+  for (int s = seg_begin[blockIdx.x]; s < seg_begin[blockIdx.x + 1]; ++s) {
+    const Seg sg = segs[s];
+    float* a = acc + sg.arena_off;
+    switch (pk.dtype[sg.tensor]) {
+      case kF32:  accum_seg<kFold, float>(reinterpret_cast<float*>(pk.ptr[sg.tensor]) + sg.src_off, a, sg.len); break;
+      case kBF16: accum_seg<kFold, __nv_bfloat16>(reinterpret_cast<__nv_bfloat16*>(pk.ptr[sg.tensor]) + sg.src_off, a, sg.len); break;
+      default:    accum_seg<kFold, __half>(reinterpret_cast<__half*>(pk.ptr[sg.tensor]) + sg.src_off, a, sg.len); break;
+    }
+  }
+}
+
+__global__ void __launch_bounds__(kThreads) grad_accumulate_kernel(const __grid_constant__ PtrPack pk, const int32_t* __restrict__ seg_begin,
+                                                                   const Seg* __restrict__ segs, float* __restrict__ acc) {
+  accum_block<false>(pk, seg_begin, segs, acc);
+}
+
+__global__ void __launch_bounds__(kThreads) grad_fold_kernel(const __grid_constant__ PtrPack pk, const int32_t* __restrict__ seg_begin,
+                                                             const Seg* __restrict__ segs, float* __restrict__ acc) {
+  accum_block<true>(pk, seg_begin, segs, acc);
+}
+
 // ================================================================= host launchers
 static void fill_ptrs(PtrPack& pk, const std::vector<at::Tensor>& ts) {
   TORCH_CHECK((int)ts.size() <= kMaxPtrs, "too many tensors in one plan launch: ", ts.size(), " > ", kMaxPtrs);
@@ -669,6 +760,28 @@ void launch_plan(const CommCtx& ctx, int kind, int wire_dtype, bool nvls, int gr
     case kF16:  nvls ? launch_kind<__half, true>(kind, grid, st, ctx, pk, a) : launch_kind<__half, false>(kind, grid, st, ctx, pk, a); break;
     default:    nvls ? launch_kind<float, true>(kind, grid, st, ctx, pk, a) : launch_kind<float, false>(kind, grid, st, ctx, pk, a); break;
   }
+  C10_CUDA_KERNEL_LAUNCH_CHECK();
+}
+
+void grad_accum(const std::vector<at::Tensor>& grads, const at::Tensor& seg_begin, const at::Tensor& segs, int64_t grid, int64_t split,
+                at::Tensor acc, int64_t acc_off, int64_t region_elems, bool fold) {
+  TORCH_CHECK(grid >= 1 && split >= 1 && split <= 65535, "grad_accum: grid out of range");
+  TORCH_CHECK(seg_begin.is_cuda() && seg_begin.scalar_type() == at::kInt && seg_begin.numel() == grid + 1, "grad_accum: seg_begin must be int32[grid + 1]");
+  TORCH_CHECK(segs.is_cuda() && segs.scalar_type() == at::kByte && segs.numel() % (int64_t)sizeof(Seg) == 0, "grad_accum: segs must be a byte segment table");
+  TORCH_CHECK(acc.is_cuda() && acc.scalar_type() == at::kFloat && acc.is_contiguous() && acc.dim() == 1, "grad_accum: acc must be a flat fp32 CUDA tensor");
+  TORCH_CHECK(acc_off >= 0 && region_elems >= 0 && acc_off + region_elems <= acc.numel(), "grad_accum: bucket range outside the accumulator");
+  float* a = acc.data_ptr<float>() + acc_off;
+  TORCH_CHECK((reinterpret_cast<uintptr_t>(a) & 31) == 0, "grad_accum: the bucket's accumulator slice must be 32-byte aligned");
+  PtrPack pk;
+  fill_ptrs(pk, grads);
+  for (const auto& g : grads) TORCH_CHECK(g.device() == acc.device(), "grad_accum: gradients and accumulator on different devices");
+  const c10::cuda::CUDAGuard guard(acc.device());
+  cudaStream_t st = at::cuda::getCurrentCUDAStream();
+  const dim3 g((unsigned)grid, (unsigned)split);
+  const auto* sb = seg_begin.data_ptr<int32_t>();
+  const auto* sg = reinterpret_cast<const Seg*>(segs.data_ptr());
+  if (fold) grad_fold_kernel<<<g, kThreads, 0, st>>>(pk, sb, sg, a);
+  else grad_accumulate_kernel<<<g, kThreads, 0, st>>>(pk, sb, sg, a);
   C10_CUDA_KERNEL_LAUNCH_CHECK();
 }
 

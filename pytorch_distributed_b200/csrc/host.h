@@ -25,6 +25,10 @@ void launch_plan(const CommCtx& ctx, int kind, int wire_dtype, bool nvls, int gr
                  int64_t seg_begin_ptr, int64_t segs_ptr, int64_t data_off_bytes, int64_t block_elems, int64_t plan_calls_ptr,
                  int64_t found_inf_ptr, double scale, bool writeback, int root, int flags = 0, int64_t result_off_bytes = -1);
 at::Tensor pack_pointers(const std::vector<at::Tensor>& tensors);
+// rank-local fp32 gradient accumulation over one bucket's plan: acc[acc_off + seg.arena_off + i] += g (fold=false), or
+// g = round(acc + g) and acc = 0 (fold=true); `split` CTAs share each plan CTA's segments
+void grad_accum(const std::vector<at::Tensor>& grads, const at::Tensor& seg_begin, const at::Tensor& segs, int64_t grid, int64_t split,
+                at::Tensor acc, int64_t acc_off, int64_t region_elems, bool fold);
 void launch_barrier(const CommCtx& ctx);
 void launch_metrics(const CommCtx& ctx, const at::Tensor& logits, const at::Tensor& target, const c10::optional<at::Tensor>& loss,
                     int64_t ll_seq_ptr, at::Tensor out);

@@ -13,6 +13,7 @@ Output contract (progress lines, `` * Acc@1`` summary, checkpoint files) is the 
 """
 from __future__ import annotations
 
+import contextlib
 import csv
 import json
 import os
@@ -194,6 +195,12 @@ class TrainStep:
     kernels are fused (bench.py reports host_enqueue_ms_per_step).  Everything the graph needs to vary is
     device-resident: hyper-parameters and loss scale (FusedSGD.hyper), signal sequence numbers (csrc/common.cuh), BN
     accumulators.  Batches of another shape (last partial batch) fall back to the eager path.
+
+    Gradient accumulation (``st.accum_steps`` = N > 1, ``--accum-steps``): one call is one micro-batch, and every N-th call
+    ends an optimizer step.  Calls 1..N-1 of a step run forward, metrics and a backward of loss / N under the strategy's
+    no-sync context; call N runs the body above with loss / N.  The metrics keep the undivided loss.  Under a graph each
+    of the two kinds of pass is captured the first time it comes after the warm-up and one eager optimizer step (two
+    graphs, one memory pool).
     """
 
     def __init__(self, st, model, criterion, optimizer, metrics, use_graph: bool = False, warmup: int = 3):
@@ -201,7 +208,12 @@ class TrainStep:
         self.use_graph = bool(use_graph) and torch.cuda.is_available()
         self.warmup = warmup
         self.calls = 0
-        self.graph = None
+        self.accum = max(1, int(getattr(st, "accum_steps", 1) or 1))
+        self.k = 0                      # pass index inside the current optimizer step
+        self.eager_steps = 0            # optimizer steps run eagerly (the first one creates the optimizer's device state)
+        self.graph = None               # the last pass of a step (the whole step without accumulation)
+        self.graph_accum = None         # the earlier passes of a step (accumulation only)
+        self.graph_launches = self.graph_accum_launches = 0
         self.static_x = self.static_y = self.static_m = None
 
     def _body(self, images, target, dev=None):
@@ -217,11 +229,20 @@ class TrainStep:
         eng = getattr(self.st, "engine", None)
         if eng is not None and getattr(eng, "bucket_view", False):
             eng.zero_grads()           # bucket views: ONE memset of the arena; backward then accumulates in place (no pack pass)
-        elif dev is None:
+        elif dev is None and self.k == 0:
             self.optimizer.zero_grad()
         if nvtx:
             torch.cuda.nvtx.range_pop()
             torch.cuda.nvtx.range_push("ptd.backward")
+        if self.accum > 1:
+            loss = loss / self.accum
+            if self.k < self.accum - 1:
+                with self.st.no_sync(self.model):
+                    self.st.backward(loss, self.optimizer, last=False)
+                if nvtx:
+                    torch.cuda.nvtx.range_pop()
+                self.metrics.join()
+                return
         self.st.backward(loss, self.optimizer)
         if nvtx:
             torch.cuda.nvtx.range_pop()
@@ -239,35 +260,53 @@ class TrainStep:
             for off, p in zip(eng.param_elem_off, eng.params):
                 arena[off:off + p.numel()].fill_(float("nan"))
 
-    def _capture(self, images, target):
-        self.static_x, self.static_y = images.clone(), target.clone()
-        self.static_m = torch.zeros(4, dtype=torch.float32, device=images.device)
-        self.optimizer.zero_grad(set_to_none=True)
+    def _static_fits(self, images):
+        return self.static_x is None or (images.shape == self.static_x.shape and images.dtype == self.static_x.dtype)
+
+    def _capture(self, images, target, last):
+        if self.static_x is None:       # both graphs read the same static batch and write the same metric vector
+            self.static_x, self.static_y = images.clone(), target.clone()
+            self.static_m = torch.zeros(4, dtype=torch.float32, device=images.device)
+        if self.k == 0:
+            self.optimizer.zero_grad(set_to_none=True)
         torch.cuda.synchronize()
         from . import _ext
         n0 = _ext.launches
         g = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(g):
+        other = self.graph_accum if last else self.graph
+        with torch.cuda.graph(g, pool=other.pool() if other is not None else None):
             self._body(self.static_x, self.static_y, self.static_m)
-        self.graph = g
-        self.graph_launches = _ext.launches - n0      # native kernels inside the graph (capture enqueues, replay runs them)
+        n = _ext.launches - n0          # native kernels inside the graph (capture enqueues, replay runs them)
         _ext.launches = n0
+        if last:
+            self.graph, self.graph_launches = g, n
+        else:
+            self.graph_accum, self.graph_accum_launches = g, n
 
     def __call__(self, images, target):
         self.calls += 1
-        if self.use_graph and self.graph is None and self.calls > self.warmup and images.is_cuda:
-            self._capture(images, target)
-        if self.graph is not None and images.shape == self.static_x.shape and images.dtype == self.static_x.dtype:
+        last = self.k == self.accum - 1
+        # with accumulation, capture after one eager optimizer step (it creates the optimizer's device state, a host copy
+        # no capture may hold) and the earlier-pass graph first: a last pass that adds into p.grad through autograd
+        # (horovod's backward_passes_per_step) must be captured reading the gradients that graph writes
+        ready = self.accum == 1 or (self.eager_steps > 0 and (not last or self.graph_accum is not None))
+        if (self.use_graph and ready and (self.graph if last else self.graph_accum) is None and self.calls > self.warmup
+                and images.is_cuda and self._static_fits(images)):
+            self._capture(images, target, last)
+        graph, launches = (self.graph, self.graph_launches) if last else (self.graph_accum, self.graph_accum_launches)
+        if graph is not None and self._static_fits(images):
             self.static_x.copy_(images, non_blocking=True)
             self.static_y.copy_(target, non_blocking=True)
-            if hasattr(self.optimizer, "refresh_hyper"):
+            if last and hasattr(self.optimizer, "refresh_hyper"):
                 self.optimizer.refresh_hyper()
-            self.graph.replay()
+            graph.replay()
             from . import _ext
-            _ext.note_launch(self.graph_launches)
+            _ext.note_launch(launches)
             self.metrics.fetch(self.static_m, images.size(0))
         else:
             self._body(images, target)
+            self.eager_steps += last
+        self.k = 0 if last else self.k + 1
         self.metrics.poll()
 
 
@@ -332,6 +371,14 @@ class Strategy:
         self.input_dtype = _DTYPES[prec] if (prec != "fp32" and self.autocast is None) else torch.float32
         return model
 
+    def set_accum_steps(self, args) -> int:
+        self.accum_steps = int(getattr(args, "accum_steps", 1) or 1)
+        return self.accum_steps
+
+    def no_sync(self, model):
+        """Context of the backwards that only accumulate (every micro-batch of an optimizer step but the last)."""
+        return model.no_sync() if hasattr(model, "no_sync") else contextlib.nullcontext()
+
     def make_optimizer(self, model, args):
         if args.optimizer == "fused":
             from .ops.fused_sgd import FusedSGD
@@ -349,7 +396,8 @@ class Strategy:
         wire = args.wire_dtype if device.type == "cuda" else "fp32"
         model = DistributedDataParallel(model, device_ids=[local_rank] if device.type == "cuda" else None,
                                         comm=self.comm_kind(args, device), wire_dtype=wire, bucket_cap_mb=args.bucket_cap_mb,
-                                        gradient_as_bucket_view=bool(getattr(args, "bucket_view", False)) and device.type == "cuda")
+                                        gradient_as_bucket_view=bool(getattr(args, "bucket_view", False)) and device.type == "cuda",
+                                        fp32_grad_accumulation=self.set_accum_steps(args) > 1)
         self.comm = model.comm
         self.engine = model.engine
         from .utils.dist_ops import set_default_communicator
@@ -368,7 +416,7 @@ class Strategy:
                 return model(images)
         return model(images)
 
-    def backward(self, loss, optimizer):
+    def backward(self, loss, optimizer, last: bool = True):
         loss.backward()
 
     def unwrapped(self, model):
@@ -405,15 +453,18 @@ class ApexStrategy(Strategy):
         wire = "fp32" if device.type != "cuda" or opt_level == "O0" else ("fp16" if half == torch.float16 else "bf16")
         if args.wire_dtype != "bf16":   # explicit override
             wire = args.wire_dtype
-        model = ApexDDP(model, comm=self.comm_kind(args, device), wire_dtype=wire)
+        model = ApexDDP(model, comm=self.comm_kind(args, device), wire_dtype=wire,
+                        fp32_grad_accumulation=self.set_accum_steps(args) > 1)
         self.comm = model.comm
         self.engine = model.engine
         self.autocast = None            # amp wrapped the forward already
         self.input_dtype = half if opt_level in ("O2", "O3") else torch.float32
         return model, optimizer
 
-    def backward(self, loss, optimizer):
-        with self.amp.scale_loss(loss, optimizer) as scaled_loss:
+    def backward(self, loss, optimizer, last: bool = True):
+        # apex's accumulation idiom: the earlier micro-batches leave their gradients scaled; an overflow in any of them
+        # reaches the last pass's sum as inf / NaN, and the step is skipped once
+        with self.amp.scale_loss(loss, optimizer, delay_unscale=not last) as scaled_loss:
             scaled_loss.backward()
 
 
@@ -449,7 +500,14 @@ class HorovodStrategy(Strategy):
         comp = {"none": hvd.Compression.none, "fp16": hvd.Compression.fp16, "bf16": hvd.Compression.bf16}[args.compression]
         if device.type != "cuda":
             comp = hvd.Compression.none
-        optimizer = hvd.DistributedOptimizer(optimizer, named_parameters=model.named_parameters(), compression=comp)
+        # --accum-steps N: horovod's own backward_passes_per_step (the gradients add up in p.grad, reduced every N-th pass)
+        n = self.set_accum_steps(args)
+        if n > 2:
+            # the gradients accumulate in p.grad through autograd, which a replayed graph cannot continue from a pass
+            # captured with p.grad already set (first pass of a step) or not (the others): keep such steps eager
+            self.graph_capable = False
+        optimizer = hvd.DistributedOptimizer(optimizer, named_parameters=model.named_parameters(), compression=comp,
+                                             backward_passes_per_step=n)
         self.comm = hvd.communicator()
         self.engine = getattr(optimizer, "_ptd_engine_obj", None)
         return model, optimizer
@@ -475,6 +533,8 @@ class DataParallelStrategy(Strategy):
         else:
             gpus = list(range(torch.cuda.device_count())) if device.type == "cuda" else []
         model = self.prepare_model(model, args, device)
+        if self.set_accum_steps(args) > 1:
+            raise ValueError("--accum-steps needs one process per GPU; DataParallel does not support it")
         model = DataParallel(model, device_ids=gpus, output_device=gpus[0] if gpus else None,
                              compute_dtype=self.input_dtype if self.autocast is None else None)
         self.comm = None
@@ -652,7 +712,13 @@ def train(train_loader, model, criterion, optimizer, epoch, st: Strategy, device
     losses = AverageMeter("Loss", ":.4e")
     top1 = AverageMeter("Acc@1", ":6.2f")
     top5 = AverageMeter("Acc@5", ":6.2f")
-    pf = st.prefetcher(train_loader, device, args, limit=args.steps_per_epoch)
+    accum = int(getattr(args, "accum_steps", 1) or 1)
+    limit = args.steps_per_epoch
+    if accum > 1:
+        # whole optimizer steps only: a group of micro-batches never crosses an epoch (or the checkpoint written after it)
+        n = len(train_loader) if limit is None else min(len(train_loader), limit)
+        limit = n // accum * accum
+    pf = st.prefetcher(train_loader, device, args, limit=limit)
     progress = ProgressMeter(len(pf), [batch_time, data_time, losses, top1, top5], prefix="Epoch: [{}]".format(epoch))
     metrics = MetricPipeline(getattr(st, "comm", None), device, (losses, top1, top5), reduce=st.reduce_metrics)
     model.train()
@@ -671,7 +737,7 @@ def train(train_loader, model, criterion, optimizer, epoch, st: Strategy, device
     step.metrics = metrics
     end = time.time()
     t0 = end
-    n_img = 0
+    n_img = n_batches = 0
     comm = getattr(st, "comm", None)
     timer = _DeviceStepTimer(device)
     kill_at = _test_kill_step(st)
@@ -680,6 +746,7 @@ def train(train_loader, model, criterion, optimizer, epoch, st: Strategy, device
             data_time.update(time.time() - end)
             step(images, target)
             n_img += images.size(0)
+            n_batches += 1
             if not timer.enabled:
                 batch_time.update(time.time() - end)      # CPU: the loop is synchronous, host time is step time
             end = time.time()
@@ -702,8 +769,11 @@ def train(train_loader, model, criterion, optimizer, epoch, st: Strategy, device
         _raise_with_comm_diagnosis(st, e)
     if device.type == "cuda":
         torch.cuda.synchronize(device)
-    _log_jsonl(args, {"phase": "train", "epoch": epoch, "rank": st.rank() if st.distributed else 0, "images": n_img,
-                      "seconds": time.time() - t0, "loss": losses.avg, "acc1": top1.avg, "acc5": top5.avg})
+    rec = {"phase": "train", "epoch": epoch, "rank": st.rank() if st.distributed else 0, "images": n_img,
+           "seconds": time.time() - t0, "loss": losses.avg, "acc1": top1.avg, "acc5": top5.avg}
+    if accum > 1:
+        rec.update(accum_steps=accum, optimizer_steps=n_batches // accum)
+    _log_jsonl(args, rec)
     return losses.avg
 
 

@@ -104,8 +104,9 @@ class FusedSGD(Optimizer):
         and push the hyper-parameters to the device before the side stream forks off."""
         if self._ov_active and self._ov_applied:
             raise RuntimeError("FusedSGD(overlap_backward=True): a second backward pass started before step() - the update of the "
-                               "previous pass has already been applied bucket by bucket; use overlap_backward=False "
-                               "(--no-overlap-optimizer) for gradient accumulation")
+                               "previous pass has already been applied bucket by bucket; accumulate gradients with the "
+                               "engine's fp32_grad_accumulation=True and no_sync() (--accum-steps), which keeps the per-bucket "
+                               "update, or use overlap_backward=False (--no-overlap-optimizer)")
         self._ov_applied = 0
         self._ov_active = self._flat is not None and self._amp is None
         if self._ov_active:
@@ -238,6 +239,7 @@ class FusedSGD(Optimizer):
                 loss = closure()
         first = self._steps == 0
         amp = self._amp
+        self._check_no_pending_accumulation()
         if self._flat is None and not self._bind_refused:
             # the engine may have been created after this optimizer (apex order: amp -> DDP), and a resumed optimizer
             # has _steps > 0 before its first step: bind whenever still unbound (existing momentum is carried over)
@@ -272,6 +274,19 @@ class FusedSGD(Optimizer):
                 amp.update()
         self._steps += 1
         return loss
+
+    def _check_no_pending_accumulation(self):
+        """An engine with fp32_grad_accumulation keeps no_sync passes in its accumulator until a synchronising backward
+        folds them in: a step before that would apply the previous step's gradients (flat) or none at all."""
+        if self._flat is not None:
+            engines = (self._flat.engine,)
+        else:
+            refs = {getattr(p, "_ptd_engine", None) for g in self.param_groups for p in g["params"]}
+            engines = [ref() for ref in refs if ref is not None]
+        for eng in engines:
+            if eng is not None and getattr(eng, "accum_pending", False):
+                raise RuntimeError("FusedSGD.step(): the gradient engine holds accumulated no_sync() passes that no synchronising "
+                                   "backward has reduced yet - run the last micro-batch's backward outside no_sync() first")
 
     def _step_group(self, gi, group, first, amp):
         params = [p for p in group["params"] if p.grad is not None]

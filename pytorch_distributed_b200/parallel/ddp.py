@@ -31,6 +31,9 @@ from ..utils.tensors import is_dense
 from .comm import KIND_ONE_SHOT, KIND_TWO_SHOT, FusedCommunicator, make_communicator
 
 _WIRE_OF = {torch.float32: "fp32", torch.bfloat16: "bf16", torch.float16: "fp16"}
+# CTAs of one grad_accumulate / grad_fold launch (the bucket plan's CTAs, each split over several): few enough to leave the
+# SMs to the backward kernels the accumulation overlaps, enough to stream the bucket at a good share of HBM bandwidth
+ACCUM_CTAS = int(os.environ.get("PTD_ACCUM_CTAS", "64"))
 
 
 class _FlatState:
@@ -70,7 +73,11 @@ class GradientEngine:
         accumulating backward leaves nothing to pack - K1 runs barrier -> multimem.ld_reduce/st -> barrier with the
         1/world scale applied to the reduced values;
       * with a bound flat optimizer in overlap mode the SGD update of the bucket's slice is enqueued right behind its
-        all-reduce, so only the small tail bucket's all-reduce + update remain after the last gradient.
+        all-reduce, so only the small tail bucket's all-reduce + update remain after the last gradient;
+      * ``fp32_grad_accumulation=True`` (extension): a backward inside ``no_sync()`` adds each ready bucket's gradients
+        into a rank-local fp32 accumulator with the arena's element layout (``grad_accumulate``, side stream) and drops
+        ``p.grad``; the next synchronising backward folds the sum into each bucket's gradients (``grad_fold``, which also
+        clears the accumulator) right before its all-reduce.  Nothing crosses GPUs before that last pass.
     """
 
     supports_flat_optimizer = True
@@ -79,7 +86,7 @@ class GradientEngine:
     def __init__(self, params: List[torch.nn.Parameter], comm, wire_dtype: str = "bf16", bucket_cap_mb: float = 25.0,
                  first_bucket_mb: float = 1.0, max_ctas: Optional[int] = None, check_inf: bool = False, average: bool = True,
                  order: str = "reverse", tail_bucket_mb: Optional[float] = 1.0, bucket_view: bool = False,
-                 delay_allreduce: bool = False, scale: Optional[float] = None):
+                 delay_allreduce: bool = False, scale: Optional[float] = None, fp32_grad_accumulation: bool = False):
         self.comm = comm
         self.world = comm.world
         self.fused = isinstance(comm, FusedCommunicator)
@@ -90,6 +97,9 @@ class GradientEngine:
         self.scale = scale if scale is not None else ((1.0 / self.world) if average else 1.0)
         self.writeback = True           # flipped off when a flat FusedSGD consumes the arena directly / with bucket views
         self.enabled = True             # no_sync()
+        self.fp32_accum = bool(fp32_grad_accumulation)
+        self._accumulating = False      # the running backward is a no_sync pass that adds into the fp32 accumulator
+        self.accum_pending = False      # the accumulator holds passes that no synchronising backward has folded yet
         self.delay_allreduce = delay_allreduce
         self.bucket_view = bool(bucket_view) and self.fused
         self._flat: Optional[_FlatState] = None
@@ -161,6 +171,16 @@ class GradientEngine:
         else:
             self.stream = None
             self.total_elems = 0
+        self._acc = None
+        if self.fp32_accum:
+            if self.fused:
+                self._acc = torch.zeros(self.total_elems, dtype=torch.float32, device=comm.device)
+            else:               # library collectives: the same sum with torch ops, parameters back to back
+                offs = [0]
+                for p in self.params:
+                    offs.append(offs[-1] + p.numel())
+                self._acc = torch.zeros(offs[-1], dtype=torch.float32, device=self.params[0].device)
+                self._acc_views = [self._acc[o:o + p.numel()].view(p.shape) for o, p in zip(offs, self.params)]
         ref = weakref.ref(self)
         self._hooks = []
         for pid, p in enumerate(self.params):
@@ -224,11 +244,12 @@ class GradientEngine:
     # ------------------------------------------------------------------ backward-time machinery
     def _make_hook(self, pid):
         def hook(param):
-            if not self.enabled:
+            if not self.enabled and not self.fp32_accum:
                 return
             if not self._callback_queued:
                 torch.autograd.Variable._execution_engine.queue_callback(self._finalize)
                 self._callback_queued = True
+                self._accumulating = not self.enabled
             b = self.bucket_of[pid]
             b.pending -= 1
             if b.pending == 0 and not self.delay_allreduce:
@@ -257,8 +278,39 @@ class GradientEngine:
             grads.append(g)
         return grads
 
+    def _accumulate(self, b, grads, fold: bool):
+        """``grad_accumulate`` (acc += g) or ``grad_fold`` (g = round(acc + g), acc = 0) over one bucket, on the current stream."""
+        if self.fused:
+            from .. import _ext
+            _ext.note_launch()
+            fn = _ext.lib().grad_fold if fold else _ext.lib().grad_accumulate
+            pl = b.plan
+            fn(grads, pl.seg_begin, pl.segs, pl.grid, max(1, ACCUM_CTAS // pl.grid), self._acc, b.elem_off, b.region_elems)
+            return
+        with torch.no_grad():
+            for pid, g in zip(b.param_ids, grads):
+                acc = self._acc_views[pid]
+                if fold:
+                    g.copy_((acc + g.float()).to(g.dtype))
+                    acc.zero_()
+                else:
+                    acc.add_(g.float())
+
     def _launch(self, b):
         grads = self._bucket_grads(b)
+        if self._accumulating:
+            if self.fused:
+                ev = torch.cuda.Event()
+                ev.record()
+                self.stream.wait_event(ev)
+                with torch.cuda.stream(self.stream):
+                    self._accumulate(b, grads, fold=False)
+                self._keepalive.append(grads)       # read on the side stream: released after the end-of-backward join
+            else:
+                self._accumulate(b, grads, fold=False)
+            b.launched = True
+            return
+        fold = self.accum_pending
         if self.fused:
             # bucket views + in-place accumulation: every gradient already sits in its arena slot => nothing to pack
             prepacked = (b.views is not None and not b.one_shot
@@ -270,6 +322,8 @@ class GradientEngine:
             ev.record()
             self.stream.wait_event(ev)
             with torch.cuda.stream(self.stream):
+                if fold:
+                    self._accumulate(b, grads, fold=True)
                 esz = P.WIRE_BYTES[self.wire]
                 self.comm.run(b.plan, grads, KIND_ONE_SHOT if b.one_shot else KIND_TWO_SHOT, self.channel, scale=self.scale,
                               writeback=self.writeback, check_inf=self.check_inf, prepacked=prepacked,
@@ -285,6 +339,8 @@ class GradientEngine:
                 for pid, v in zip(b.param_ids, b.views):    # torch semantics: after the reduction p.grad IS the bucket view
                     self.params[pid].grad = v
         else:
+            if fold:
+                self._accumulate(b, grads, fold=True)
             fin = self.comm.all_reduce_(grads, average=self.average, wire=self.wire, async_op=True)
             if fin is not None:
                 self._pending_finish.append(fin)
@@ -311,6 +367,14 @@ class GradientEngine:
             b.pending = len(b.param_ids)
             b.launched = False
         self._next_bucket = 0
+        if self._accumulating:
+            # the pass lives in the accumulator now: a later backward must not add it again through p.grad
+            for p in self.params:
+                p.grad = None
+            self._accumulating = False
+            self.accum_pending = True
+        else:
+            self.accum_pending = False
 
     def wait_for_gradients(self):
         if self._grads_ready_event is not None and not torch.cuda.is_current_stream_capturing():
@@ -368,7 +432,9 @@ class DistributedDataParallel(nn.Module):
     Constructor arguments with torch's meaning: ``device_ids`` (checked against the module's device), ``broadcast_buffers``,
     ``process_group``, ``bucket_cap_mb``, ``gradient_as_bucket_view`` (``p.grad`` become views of the symmetric arena: no
     write-back pass, and no pack pass either when the gradients are accumulated in place - ``zero_grad(set_to_none=False)``
-    or ``engine.zero_grads()``).  ``find_unused_parameters`` is accepted and always effectively on: a bucket whose
+    or ``engine.zero_grads()``).  ``fp32_grad_accumulation`` (extension): backwards inside ``no_sync()`` sum into an fp32
+    buffer instead of ``p.grad`` (which they leave None); the next backward outside it folds the sum in and reduces it.
+    ``find_unused_parameters`` is accepted and always effectively on: a bucket whose
     parameters did not all receive a gradient is flushed at the end of backward with zeros for the missing ones, no
     graph traversal needed.  ``output_device`` / ``dim`` other than the module's device / 0 are rejected (single-device
     module replicas only, like the reference's use).
@@ -377,7 +443,8 @@ class DistributedDataParallel(nn.Module):
     def __init__(self, module: nn.Module, device_ids=None, output_device=None, dim=0, broadcast_buffers: bool = True,
                  process_group=None, bucket_cap_mb: float = 25.0, find_unused_parameters: bool = False,
                  gradient_as_bucket_view: bool = False, comm="auto", wire_dtype: Optional[str] = None, max_ctas: Optional[int] = None,
-                 check_inf: bool = False, tail_bucket_mb: Optional[float] = 1.0, deferred_buffer_broadcast: Optional[bool] = None):
+                 check_inf: bool = False, tail_bucket_mb: Optional[float] = 1.0, deferred_buffer_broadcast: Optional[bool] = None,
+                 fp32_grad_accumulation: bool = False):
         super().__init__()
         self.module = module
         params = [p for p in module.parameters() if p.requires_grad]
@@ -411,7 +478,8 @@ class DistributedDataParallel(nn.Module):
                 wire_dtype = "bf16" if self.device.type == "cuda" else "fp32"
         sync_module_states(module, comm, root=0)
         self.engine = GradientEngine(params, comm, wire_dtype=wire_dtype, bucket_cap_mb=bucket_cap_mb, max_ctas=max_ctas,
-                                     check_inf=check_inf, tail_bucket_mb=tail_bucket_mb, bucket_view=gradient_as_bucket_view)
+                                     check_inf=check_inf, tail_bucket_mb=tail_bucket_mb, bucket_view=gradient_as_bucket_view,
+                                     fp32_grad_accumulation=fp32_grad_accumulation)
         self._buffers_f = _float_buffers(module)
         # torch re-broadcasts rank 0's buffers BEFORE every forward, on the compute stream: a cross-GPU barrier at the top of
         # each step.  Deferred mode broadcasts rank 0's buffers right AFTER the forward that updated them, on the side stream

@@ -23,6 +23,10 @@ KERNELS = [
     (r"barrier_kernel", "barrier_kernel", "collectives.cu", "K3", "tests/mp_gpu_checks.py"),
     (r"fused_sgd_flat_kernelI13__nv_bfloat16S1_Lb1E", "fused_sgd_flat_kernel<bf16 grad, bf16 model>", "optim.cu",
      "K6: unscale + overflow skip + SGD momentum over arena / fp32 masters / momentum / bf16 copy", "tests/test_gpu_kernels.py"),
+    (r"grad_accumulate_kernel", "grad_accumulate_kernel", "collectives.cu",
+     "--accum-steps: bucket gradients added into the rank-local fp32 sum (no_sync passes)", "tests/test_gpu_grad_accum.py, tools/accum_bench.py"),
+    (r"grad_fold_kernel", "grad_fold_kernel", "collectives.cu",
+     "--accum-steps: fp32 sum folded into the last pass's gradients and cleared, before K1", "tests/test_gpu_grad_accum.py, tools/accum_bench.py"),
     (r"fused_sgd_multi_kernel", "fused_sgd_multi_kernel", "optim.cu", "multi-tensor-apply variant (non-flat parameters)", "tests/test_gpu_kernels.py"),
     (r"larc_norm_flat_kernelI13__nv_bfloat16E", "larc_norm_flat_kernel<bf16>", "optim.cu",
      "LARC norm pass: per-chunk fp32 sums of p^2 and (g gmul)^2 over the arena, fixed order", "tests/test_gpu_larc.py, tools/larc_bench.py"),
