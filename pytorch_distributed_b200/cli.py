@@ -100,6 +100,11 @@ def build_parser(entry: str = "distributed") -> argparse.ArgumentParser:
     x.add_argument("--accum-steps", default=1, type=_positive_int, metavar="N",
                    help="gradient accumulation: one optimizer step per N consecutive batches (effective batch -b x N); the fused "
                         "engine sums the earlier passes in fp32 on each GPU and reduces once, in the last pass (default: 1)")
+    x.add_argument("--model-ema", action="store_true",
+                   help="keep an exponential moving average of the weights (fp32, updated inside the fused optimizer step), "
+                        "validate it after each epoch and save it as state_dict_ema")
+    x.add_argument("--model-ema-decay", default=None, type=float, metavar="D",
+                   help="decay of --model-ema: e = D e + (1 - D) p after every optimizer step, 0 <= D < 1 (default: 0.9999)")
     x.add_argument("--cuda-graph", action="store_true", help="capture the train step in a CUDA graph")
     x.add_argument("--sync-bn", action="store_true",
                    help="synchronise BatchNorm statistics across the data-parallel ranks (torch.nn.SyncBatchNorm semantics; "
@@ -147,6 +152,10 @@ def parse_args(entry: str, argv=None):
     args = parser.parse_args(argv)
     if not args.larc and (args.larc_trust_coefficient is not None or args.larc_clip is not None):
         parser.error("--larc-trust-coefficient / --larc-clip / --no-larc-clip need --larc")
+    if not args.model_ema and args.model_ema_decay is not None:
+        parser.error("--model-ema-decay needs --model-ema")
+    if args.model_ema_decay is not None and not (0.0 <= args.model_ema_decay < 1.0):
+        parser.error("--model-ema-decay must lie in [0, 1), got %r" % (args.model_ema_decay,))
     if args.accum_steps > 1 and entry == "dataparallel":
         parser.error("--accum-steps needs one process per GPU; the single-process DataParallel entrypoint does not support it")
     if args.steps_per_epoch is not None and args.steps_per_epoch < args.accum_steps:
@@ -156,5 +165,7 @@ def parse_args(entry: str, argv=None):
         args.larc_trust_coefficient = 0.02
     if args.larc_clip is None:
         args.larc_clip = True
+    if args.model_ema_decay is None:
+        args.model_ema_decay = 0.9999
     args.entry = entry
     return args

@@ -116,15 +116,18 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("grads"), py::arg("seg_begin"), py::arg("segs"), py::arg("grid"), py::arg("split"), py::arg("acc"), py::arg("acc_off"),
         py::arg("region_elems"));
   m.def("fused_sgd_flat", &fused_sgd_flat, py::arg("grad"), py::arg("master"), py::arg("momentum"), py::arg("model_copy"), py::arg("hyper"),
-        py::arg("found_inf"), py::arg("nesterov"), py::arg("first_step"));
-  m.def("fused_sgd_multi", &fused_sgd_multi);
+        py::arg("found_inf"), py::arg("nesterov"), py::arg("first_step"), py::arg("ema") = c10::optional<at::Tensor>());
+  m.def("fused_sgd_multi", &fused_sgd_multi, py::arg("grads"), py::arg("params"), py::arg("momenta"), py::arg("model_copies"),
+        py::arg("hyper"), py::arg("found_inf"), py::arg("nesterov"), py::arg("first_step"), py::arg("ema") = std::vector<at::Tensor>());
+  m.def("ema_multi", &ema_multi, py::arg("src"), py::arg("dst"), py::arg("dw"), py::arg("found_inf") = c10::optional<at::Tensor>());
   m.attr("LARC_CHUNK") = kLarcChunkElems;
   m.def("larc_sgd_flat", &larc_sgd_flat, py::arg("grad"), py::arg("master"), py::arg("momentum"), py::arg("model_copy"), py::arg("hyper"),
         py::arg("found_inf"), py::arg("nesterov"), py::arg("first_step"), py::arg("chunk_tensor"), py::arg("info"), py::arg("chunk_lo"),
-        py::arg("chunk_hi"), py::arg("partials"), py::arg("stats"), py::arg("trust"), py::arg("eps"), py::arg("clip"));
+        py::arg("chunk_hi"), py::arg("partials"), py::arg("stats"), py::arg("trust"), py::arg("eps"), py::arg("clip"),
+        py::arg("ema") = c10::optional<at::Tensor>());
   m.def("larc_sgd_multi", &larc_sgd_multi, py::arg("grads"), py::arg("params"), py::arg("momenta"), py::arg("model_copies"), py::arg("hyper"),
         py::arg("found_inf"), py::arg("nesterov"), py::arg("first"), py::arg("rows"), py::arg("stats"), py::arg("trust"), py::arg("eps"),
-        py::arg("clip"));
+        py::arg("clip"), py::arg("ema") = std::vector<at::Tensor>());
   m.def("multi_tensor_scale", &multi_tensor_scale);
   m.def("multi_tensor_axpby", &multi_tensor_axpby);
   m.def("amp_update_scale", &amp_update_scale);

@@ -35,11 +35,14 @@ void launch_metrics(const CommCtx& ctx, const at::Tensor& logits, const at::Tens
 void launch_ll_allreduce(const CommCtx& ctx, const at::Tensor& in, at::Tensor out, double scale, int64_t ll_seq_ptr);
 
 // ---- optim.cu
+// `ema` (optional, ModelEma): fp32 averages updated from the new masters with the decay in hyper[6], hyper[7]
 void fused_sgd_flat(at::Tensor grad, at::Tensor master, at::Tensor momentum, c10::optional<at::Tensor> model_copy,
-                    at::Tensor hyper, c10::optional<at::Tensor> found_inf, bool nesterov, bool first_step);
+                    at::Tensor hyper, c10::optional<at::Tensor> found_inf, bool nesterov, bool first_step, c10::optional<at::Tensor> ema);
 void fused_sgd_multi(std::vector<at::Tensor> grads, std::vector<at::Tensor> params, std::vector<at::Tensor> momenta,
                      std::vector<at::Tensor> model_copies, at::Tensor hyper, c10::optional<at::Tensor> found_inf, bool nesterov,
-                     bool first_step);
+                     bool first_step, std::vector<at::Tensor> ema);
+// dst = fmaf(dw[0], dst, dw[1] * src) over tensor lists (fp32 dst), nothing when found_inf is set
+void ema_multi(std::vector<at::Tensor> src, std::vector<at::Tensor> dst, at::Tensor dw, c10::optional<at::Tensor> found_inf);
 void multi_tensor_scale(std::vector<at::Tensor> src, std::vector<at::Tensor> dst, double scale, at::Tensor found_inf);
 void multi_tensor_axpby(std::vector<at::Tensor> x, std::vector<at::Tensor> y, std::vector<at::Tensor> out, double a, double b,
                         at::Tensor found_inf);
@@ -47,10 +50,12 @@ void multi_tensor_axpby(std::vector<at::Tensor> x, std::vector<at::Tensor> y, st
 constexpr int64_t kLarcChunkElems = 8192;
 void larc_sgd_flat(at::Tensor grad, at::Tensor master, at::Tensor momentum, c10::optional<at::Tensor> model_copy, at::Tensor hyper,
                    c10::optional<at::Tensor> found_inf, bool nesterov, bool first_step, at::Tensor chunk_tensor, at::Tensor info,
-                   int64_t chunk_lo, int64_t chunk_hi, at::Tensor partials, at::Tensor stats, double trust, double eps, bool clip);
+                   int64_t chunk_lo, int64_t chunk_hi, at::Tensor partials, at::Tensor stats, double trust, double eps, bool clip,
+                   c10::optional<at::Tensor> ema);
 void larc_sgd_multi(std::vector<at::Tensor> grads, std::vector<at::Tensor> params, std::vector<at::Tensor> momenta,
                     std::vector<c10::optional<at::Tensor>> model_copies, at::Tensor hyper, c10::optional<at::Tensor> found_inf, bool nesterov,
-                    std::vector<bool> first, std::vector<int64_t> rows, at::Tensor stats, double trust, double eps, bool clip);
+                    std::vector<bool> first, std::vector<int64_t> rows, at::Tensor stats, double trust, double eps, bool clip,
+                    std::vector<at::Tensor> ema);
 void amp_update_scale(at::Tensor scale, at::Tensor growth_tracker, at::Tensor found_inf, double growth, double backoff,
                       int64_t interval, at::Tensor hyper);
 

@@ -16,6 +16,11 @@
 // momentum_pending (slot 5) is read only under dynamic loss scaling (a found_inf flag is given): while it is non-zero the
 // step initialises the momentum buffer (m = g), as on the first step.  amp_update_scale clears it after the first step
 // that was applied, so a skipped (overflowed) first step does not turn the next one into m = (1 - dampening) g.
+//
+// Exponential moving average (ModelEma): every update kernel has an HAS_EMA instantiation that also streams an fp32 average
+// e of the masters, updated from the new master p as e = fmaf(d, e, w p) with d = hyper[6] and w = hyper[7] = fp32(1 - d)
+// (+8 B/element).  d = 0 gives e = p and d = 1 leaves e unchanged, bit for bit.  The found_inf early return skips it with
+// the step.  ema_multi applies the same formula to any tensor lists (BatchNorm buffers, optimizers other than these).
 #include <ATen/cuda/CUDAContext.h>
 #include <c10/cuda/CUDAGuard.h>
 #include <torch/extension.h>
@@ -26,6 +31,9 @@
 namespace ptd {
 
 struct SgdHyper { float lr, momentum, wd, dampening, gmul; };
+struct EmaHyper { float d, w; };
+
+__device__ __forceinline__ float ema_update(float e, float p, const EmaHyper& h) { return __fmaf_rn(h.d, e, __fmul_rn(h.w, p)); }
 
 __device__ __forceinline__ SgdHyper load_hyper(const float* h) { return SgdHyper{h[0], h[1], h[2], h[3], h[4]}; }
 
@@ -38,13 +46,16 @@ __device__ __forceinline__ void sgd_update(float g, float& p, float& m, const Sg
   p -= h.lr * g;
 }
 
-template <typename G, typename C, bool HAS_COPY>
+// `ema` is the last parameter so that the HAS_EMA = false instantiations keep their parameter offsets (and SASS)
+template <typename G, typename C, bool HAS_COPY, bool HAS_EMA>
 __global__ void __launch_bounds__(256) fused_sgd_flat_kernel(const G* __restrict__ grad, float* __restrict__ master,
                                                              float* __restrict__ mom, C* __restrict__ copy, int64_t n,
                                                              const float* __restrict__ hyper, const int* __restrict__ found_inf,
-                                                             bool nesterov, bool first) {
+                                                             bool nesterov, bool first, float* __restrict__ ema) {
   if (found_inf && *found_inf) return;  // dynamic loss scaling: skip the step on overflow
   const SgdHyper h = load_hyper(hyper);
+  EmaHyper eh{};
+  if constexpr (HAS_EMA) eh = EmaHyper{hyper[6], hyper[7]};
   first = first || (found_inf && hyper[5] != 0.f);
   const int64_t nvec = n >> 3;
   for (int64_t v = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; v < nvec; v += (int64_t)gridDim.x * blockDim.x) {
@@ -57,18 +68,33 @@ __global__ void __launch_bounds__(256) fused_sgd_flat_kernel(const G* __restrict
     store8<float>(master + (v << 3), p);
     store8<float>(mom + (v << 3), m);
     if constexpr (HAS_COPY) store8<C>(copy + (v << 3), p);
+    if constexpr (HAS_EMA) {
+      float e[8];
+      load8<float>(ema + (v << 3), e);
+#pragma unroll
+      for (int k = 0; k < 8; ++k) e[k] = ema_update(e[k], p[k], eh);
+      store8<float>(ema + (v << 3), e);
+    }
   }
   // n is padded to a multiple of 8 by the arena layout; no scalar tail.
 }
 
+static void check_ema_flat(const c10::optional<at::Tensor>& ema, int64_t n, const at::Tensor& hyper) {
+  if (!ema.has_value()) return;
+  TORCH_CHECK(ema->scalar_type() == at::kFloat && ema->numel() == n && ema->is_contiguous() && ema->device() == hyper.device(),
+              "the EMA buffer must be a contiguous fp32 tensor with the masters' layout");
+  TORCH_CHECK(hyper.numel() >= 8, "hyper needs slots 6, 7 (EMA decay) when an EMA buffer is given");
+}
+
 void fused_sgd_flat(at::Tensor grad, at::Tensor master, at::Tensor momentum, c10::optional<at::Tensor> model_copy, at::Tensor hyper,
-                    c10::optional<at::Tensor> found_inf, bool nesterov, bool first_step) {
+                    c10::optional<at::Tensor> found_inf, bool nesterov, bool first_step, c10::optional<at::Tensor> ema) {
   const int64_t n = master.numel();
   TORCH_CHECK(n % 8 == 0, "flat optimizer buffers must be padded to a multiple of 8 elements");
   TORCH_CHECK(grad.numel() >= n && momentum.numel() == n, "flat buffer size mismatch");
   TORCH_CHECK(master.scalar_type() == at::kFloat && momentum.scalar_type() == at::kFloat && hyper.scalar_type() == at::kFloat);
   TORCH_CHECK(master.is_contiguous() && momentum.is_contiguous() && grad.is_contiguous());
   TORCH_CHECK(!found_inf.has_value() || hyper.numel() >= 6, "hyper needs slot 5 (momentum_pending) when found_inf is given");
+  check_ema_flat(ema, n, hyper);
   c10::cuda::CUDAGuard guard(master.device());
   const int* fi = found_inf.has_value() ? reinterpret_cast<const int*>(found_inf->data_ptr()) : nullptr;
   const int sms = at::cuda::getCurrentDeviceProperties()->multiProcessorCount;
@@ -77,8 +103,14 @@ void fused_sgd_flat(at::Tensor grad, at::Tensor master, at::Tensor momentum, c10
   float* mp = master.data_ptr<float>();
   float* vp = momentum.data_ptr<float>();
   const float* hp = hyper.data_ptr<float>();
-#define LAUNCH(G, C, HC, cptr) \
-  fused_sgd_flat_kernel<G, C, HC><<<grid, 256, 0, st>>>(reinterpret_cast<const G*>(grad.data_ptr()), mp, vp, cptr, n, hp, fi, nesterov, first_step)
+  float* ep = ema.has_value() ? ema->data_ptr<float>() : nullptr;
+#define LAUNCH(G, C, HC, cptr)                                                                                                   \
+  do {                                                                                                                          \
+    if (ep) fused_sgd_flat_kernel<G, C, HC, true><<<grid, 256, 0, st>>>(reinterpret_cast<const G*>(grad.data_ptr()), mp, vp, cptr, \
+                                                                        n, hp, fi, nesterov, first_step, ep);                  \
+    else fused_sgd_flat_kernel<G, C, HC, false><<<grid, 256, 0, st>>>(reinterpret_cast<const G*>(grad.data_ptr()), mp, vp, cptr, \
+                                                                       n, hp, fi, nesterov, first_step, nullptr);              \
+  } while (0)
   const bool has_copy = model_copy.has_value();
   if (has_copy) TORCH_CHECK(model_copy->numel() == n && model_copy->is_contiguous());
   const auto gt = grad.scalar_type();
@@ -134,11 +166,14 @@ __device__ __forceinline__ void st_any(void* p, int dt, int64_t i, float v) {
   }
 }
 
-// lists: 0 grad, 1 param (fp32 master), 2 momentum (fp32), 3 model copy (optional: ptr may be null)
-__global__ void __launch_bounds__(256) fused_sgd_multi_kernel(const __grid_constant__ MtaArgs<4> a, const float* __restrict__ hyper,
+// lists: 0 grad, 1 param (fp32 master), 2 momentum (fp32), 3 model copy (optional: ptr may be null), 4 fp32 EMA (HAS_EMA)
+template <bool HAS_EMA>
+__global__ void __launch_bounds__(256) fused_sgd_multi_kernel(const __grid_constant__ MtaArgs<HAS_EMA ? 5 : 4> a, const float* __restrict__ hyper,
                                                               const int* __restrict__ found_inf, bool nesterov, bool first) {
   if (found_inf && *found_inf) return;
   const SgdHyper h = load_hyper(hyper);
+  EmaHyper eh{};
+  if constexpr (HAS_EMA) eh = EmaHyper{hyper[6], hyper[7]};
   first = first || (found_inf && hyper[5] != 0.f);
   const int t = a.block_tensor[blockIdx.x];
   const int64_t begin = (int64_t)a.block_chunk[blockIdx.x] * kMtaChunk;
@@ -152,7 +187,24 @@ __global__ void __launch_bounds__(256) fused_sgd_multi_kernel(const __grid_const
     p[i] = pv;
     m[i] = mv;
     if (a.ptr[3][t]) st_any(a.ptr[3][t], cdt, i, pv);
+    if constexpr (HAS_EMA) {
+      float* e = reinterpret_cast<float*>(a.ptr[4][t]);
+      e[i] = ema_update(e[i], pv, eh);
+    }
   }
+}
+
+// dst = fmaf(d, dst, w * src) with {d, w} = dw[0..1] (fp32 dst, any float src); nothing on found_inf.  lists: 0 src, 1 dst
+__global__ void __launch_bounds__(256) ema_multi_kernel(const __grid_constant__ MtaArgs<2> a, const float* __restrict__ dw,
+                                                        const int* __restrict__ found_inf) {
+  if (found_inf && *found_inf) return;
+  const EmaHyper eh{dw[0], dw[1]};
+  const int t = a.block_tensor[blockIdx.x];
+  const int64_t begin = (int64_t)a.block_chunk[blockIdx.x] * kMtaChunk;
+  const int64_t end = min(begin + (int64_t)kMtaChunk, a.numel[t]);
+  float* e = reinterpret_cast<float*>(a.ptr[1][t]);
+  const int sdt = a.dtype[0][t];
+  for (int64_t i = begin + threadIdx.x; i < end; i += blockDim.x) e[i] = ema_update(e[i], ld_any(a.ptr[0][t], sdt, i), eh);
 }
 
 // dst = src * scale, found_inf |= any non-finite(src)
@@ -232,21 +284,56 @@ static void mta_for_each(const std::vector<std::vector<at::Tensor>>& lists, Laun
   flush();
 }
 
+// EMA list of a multi-tensor update: empty (no EMA) or one fp32 tensor per master, with the master's strides
+static void check_ema_multi(const std::vector<at::Tensor>& ema, const std::vector<at::Tensor>& params, const at::Tensor& hyper) {
+  if (ema.empty()) return;
+  TORCH_CHECK(ema.size() == params.size(), "the EMA list needs one tensor per parameter");
+  TORCH_CHECK(hyper.numel() >= 8, "hyper needs slots 6, 7 (EMA decay) when an EMA list is given");
+  for (size_t i = 0; i < ema.size(); ++i)
+    TORCH_CHECK(ema[i].scalar_type() == at::kFloat && ema[i].strides() == params[i].strides() && ema[i].numel() == params[i].numel(),
+                "EMA tensors must be fp32 with their master's shape and strides");
+}
+
 void fused_sgd_multi(std::vector<at::Tensor> grads, std::vector<at::Tensor> params, std::vector<at::Tensor> momenta,
                      std::vector<at::Tensor> model_copies, at::Tensor hyper, c10::optional<at::Tensor> found_inf, bool nesterov,
-                     bool first_step) {
+                     bool first_step, std::vector<at::Tensor> ema) {
   if (params.empty()) return;
   TORCH_CHECK(grads.size() == params.size() && momenta.size() == params.size());
   TORCH_CHECK(model_copies.empty() || model_copies.size() == params.size());
   for (auto& p : params) TORCH_CHECK(p.scalar_type() == at::kFloat, "params (masters) must be fp32");
   for (auto& m : momenta) TORCH_CHECK(m.scalar_type() == at::kFloat, "momentum must be fp32");
   TORCH_CHECK(!found_inf.has_value() || hyper.numel() >= 6, "hyper needs slot 5 (momentum_pending) when found_inf is given");
+  check_ema_multi(ema, params, hyper);
   c10::cuda::CUDAGuard guard(params[0].device());
   cudaStream_t st = at::cuda::getCurrentCUDAStream();
   const int* fi = found_inf.has_value() ? reinterpret_cast<const int*>(found_inf->data_ptr()) : nullptr;
   const float* hp = hyper.data_ptr<float>();
+  if (!ema.empty()) {
+    mta_for_each<5>({grads, params, momenta, model_copies, ema}, [&](const MtaArgs<5>& a, int nb, const int*) {
+      fused_sgd_multi_kernel<true><<<nb, 256, 0, st>>>(a, hp, fi, nesterov, first_step);
+      C10_CUDA_KERNEL_LAUNCH_CHECK();
+    });
+    return;
+  }
   mta_for_each<4>({grads, params, momenta, model_copies}, [&](const MtaArgs<4>& a, int nb, const int*) {
-    fused_sgd_multi_kernel<<<nb, 256, 0, st>>>(a, hp, fi, nesterov, first_step);
+    fused_sgd_multi_kernel<false><<<nb, 256, 0, st>>>(a, hp, fi, nesterov, first_step);
+    C10_CUDA_KERNEL_LAUNCH_CHECK();
+  });
+}
+
+void ema_multi(std::vector<at::Tensor> src, std::vector<at::Tensor> dst, at::Tensor dw, c10::optional<at::Tensor> found_inf) {
+  if (dst.empty()) return;
+  TORCH_CHECK(src.size() == dst.size(), "ema_multi: one source per average");
+  TORCH_CHECK(dw.scalar_type() == at::kFloat && dw.numel() >= 2 && dw.is_cuda(), "ema_multi: dw = fp32 {d, 1 - d} on the device");
+  for (size_t i = 0; i < dst.size(); ++i)
+    TORCH_CHECK(dst[i].scalar_type() == at::kFloat && dst[i].strides() == src[i].strides(),
+                "ema_multi: averages must be fp32 with their source's strides");
+  c10::cuda::CUDAGuard guard(dst[0].device());
+  cudaStream_t st = at::cuda::getCurrentCUDAStream();
+  const int* fi = found_inf.has_value() ? reinterpret_cast<const int*>(found_inf->data_ptr()) : nullptr;
+  const float* dp = dw.data_ptr<float>();
+  mta_for_each<2>({src, dst}, [&](const MtaArgs<2>& a, int nb, const int*) {
+    ema_multi_kernel<<<nb, 256, 0, st>>>(a, dp, fi);
     C10_CUDA_KERNEL_LAUNCH_CHECK();
   });
 }
@@ -430,15 +517,18 @@ __global__ void __launch_bounds__(kLarcThreads) larc_norm_flat_kernel(const G* _
   if (threadIdx.x == 0) partials[q] = s;
 }
 
-template <typename G, typename C, bool HAS_COPY>
+template <typename G, typename C, bool HAS_COPY, bool HAS_EMA>
 __global__ void __launch_bounds__(kLarcThreads) larc_sgd_flat_kernel(const G* __restrict__ grad, float* __restrict__ master, float* __restrict__ mom,
                                                                      C* __restrict__ copy, const int32_t* __restrict__ chunk_tensor,
                                                                      const int64_t* __restrict__ info, int64_t chunk_lo,
                                                                      const float2* __restrict__ partials, float* __restrict__ stats,
                                                                      const float* __restrict__ hyper, const int* __restrict__ found_inf,
-                                                                     bool nesterov, bool first, float trust, float eps, bool clip) {
+                                                                     bool nesterov, bool first, float trust, float eps, bool clip,
+                                                                     float* __restrict__ ema) {
   if (found_inf && *found_inf) return;  // dynamic loss scaling: skip the step on overflow
   const SgdHyper h = load_hyper(hyper);
+  EmaHyper eh{};
+  if constexpr (HAS_EMA) eh = EmaHyper{hyper[6], hyper[7]};
   first = first || (found_inf && hyper[5] != 0.f);
   const LarcChunk k = larc_chunk(chunk_tensor, info, chunk_lo + blockIdx.x);
   const LarcFactor r = larc_factor(partials + k.cbase, k.nchunks, h, trust, eps, clip);
@@ -456,6 +546,13 @@ __global__ void __launch_bounds__(kLarcThreads) larc_sgd_flat_kernel(const G* __
       store8<float>(master + e, p);
       store8<float>(mom + e, m);
       if constexpr (HAS_COPY) store8<C>(copy + e, p);
+      if constexpr (HAS_EMA) {
+        float a[8];
+        load8<float>(ema + e, a);
+#pragma unroll
+        for (int j = 0; j < 8; ++j) a[j] = ema_update(a[j], p[j], eh);
+        store8<float>(ema + e, a);
+      }
     } else {
       for (int64_t x = e; x < base + k.len; ++x) {
         float p = master[x], m = mom[x];
@@ -466,6 +563,7 @@ __global__ void __launch_bounds__(kLarcThreads) larc_sgd_flat_kernel(const G* __
           if constexpr (std::is_same<C, __nv_bfloat16>::value) copy[x] = __float2bfloat16_rn(p);
           else copy[x] = __float2half_rn(p);
         }
+        if constexpr (HAS_EMA) ema[x] = ema_update(ema[x], p, eh);
       }
     }
   }
@@ -497,13 +595,16 @@ __global__ void __launch_bounds__(kLarcThreads) larc_norm_multi_kernel(const __g
   if (threadIdx.x == 0) partials[s.cbase[t] + c] = r;
 }
 
-// lists: 0 grad, 1 fp32 master, 2 momentum (fp32), 3 model copy (optional: ptr may be null)
-__global__ void __launch_bounds__(kLarcThreads) larc_sgd_multi_kernel(const __grid_constant__ MtaArgs<4> a, const __grid_constant__ LarcSlots s,
+// lists: 0 grad, 1 fp32 master, 2 momentum (fp32), 3 model copy (optional: ptr may be null), 4 fp32 EMA (HAS_EMA)
+template <bool HAS_EMA>
+__global__ void __launch_bounds__(kLarcThreads) larc_sgd_multi_kernel(const __grid_constant__ MtaArgs<HAS_EMA ? 5 : 4> a, const __grid_constant__ LarcSlots s,
                                                                       const float2* __restrict__ partials, float* __restrict__ stats,
                                                                       const float* __restrict__ hyper, const int* __restrict__ found_inf,
                                                                       bool nesterov, float trust, float eps, bool clip) {
   if (found_inf && *found_inf) return;
   const SgdHyper h = load_hyper(hyper);
+  EmaHyper eh{};
+  if constexpr (HAS_EMA) eh = EmaHyper{hyper[6], hyper[7]};
   const int t = a.block_tensor[blockIdx.x];
   const bool first = s.first[t] || (found_inf && hyper[5] != 0.f);
   const int c = a.block_chunk[blockIdx.x];
@@ -520,6 +621,10 @@ __global__ void __launch_bounds__(kLarcThreads) larc_sgd_multi_kernel(const __gr
     p[i] = pv;
     m[i] = mv;
     if (a.ptr[3][t]) st_any(a.ptr[3][t], cdt, i, pv);
+    if constexpr (HAS_EMA) {
+      float* e = reinterpret_cast<float*>(a.ptr[4][t]);
+      e[i] = ema_update(e[i], pv, eh);
+    }
   }
 }
 
@@ -548,7 +653,8 @@ static void larc_flat_types(at::ScalarType gt, c10::optional<at::ScalarType> ct,
 
 void larc_sgd_flat(at::Tensor grad, at::Tensor master, at::Tensor momentum, c10::optional<at::Tensor> model_copy, at::Tensor hyper,
                    c10::optional<at::Tensor> found_inf, bool nesterov, bool first_step, at::Tensor chunk_tensor, at::Tensor info,
-                   int64_t chunk_lo, int64_t chunk_hi, at::Tensor partials, at::Tensor stats, double trust, double eps, bool clip) {
+                   int64_t chunk_lo, int64_t chunk_hi, at::Tensor partials, at::Tensor stats, double trust, double eps, bool clip,
+                   c10::optional<at::Tensor> ema) {
   const int64_t n = master.numel();
   TORCH_CHECK(grad.numel() >= n && momentum.numel() == n, "flat buffer size mismatch");
   TORCH_CHECK(master.scalar_type() == at::kFloat && momentum.scalar_type() == at::kFloat);
@@ -560,6 +666,7 @@ void larc_sgd_flat(at::Tensor grad, at::Tensor master, at::Tensor momentum, c10:
   TORCH_CHECK(partials.scalar_type() == at::kFloat && partials.is_contiguous() && partials.numel() >= 2 * chunk_tensor.numel(),
               "LARC partials: fp32 [2 * chunks]");
   if (model_copy.has_value()) TORCH_CHECK(model_copy->numel() == n && model_copy->is_contiguous());
+  check_ema_flat(ema, n, hyper);
   if (chunk_hi == chunk_lo) return;
   c10::cuda::CUDAGuard guard(master.device());
   cudaStream_t st = at::cuda::getCurrentCUDAStream();
@@ -577,16 +684,22 @@ void larc_sgd_flat(at::Tensor grad, at::Tensor master, at::Tensor momentum, c10:
                     larc_norm_flat_kernel<G><<<grid, kLarcThreads, 0, st>>>(gp, master.data_ptr<float>(), ct, inf, chunk_lo, part, hp, fi);
                     C10_CUDA_KERNEL_LAUNCH_CHECK();
                     C* cp = has_copy ? reinterpret_cast<C*>(model_copy->data_ptr()) : nullptr;
-                    larc_sgd_flat_kernel<G, C, decltype(has_copy)::value><<<grid, kLarcThreads, 0, st>>>(
-                        gp, master.data_ptr<float>(), momentum.data_ptr<float>(), cp, ct, inf, chunk_lo, part, stats.data_ptr<float>(), hp, fi,
-                        nesterov, first_step, (float)trust, (float)eps, clip);
+                    if (ema.has_value())
+                      larc_sgd_flat_kernel<G, C, decltype(has_copy)::value, true><<<grid, kLarcThreads, 0, st>>>(
+                          gp, master.data_ptr<float>(), momentum.data_ptr<float>(), cp, ct, inf, chunk_lo, part, stats.data_ptr<float>(), hp,
+                          fi, nesterov, first_step, (float)trust, (float)eps, clip, ema->data_ptr<float>());
+                    else
+                      larc_sgd_flat_kernel<G, C, decltype(has_copy)::value, false><<<grid, kLarcThreads, 0, st>>>(
+                          gp, master.data_ptr<float>(), momentum.data_ptr<float>(), cp, ct, inf, chunk_lo, part, stats.data_ptr<float>(), hp,
+                          fi, nesterov, first_step, (float)trust, (float)eps, clip, nullptr);
                     C10_CUDA_KERNEL_LAUNCH_CHECK();
                   });
 }
 
 void larc_sgd_multi(std::vector<at::Tensor> grads, std::vector<at::Tensor> params, std::vector<at::Tensor> momenta,
                     std::vector<c10::optional<at::Tensor>> model_copies, at::Tensor hyper, c10::optional<at::Tensor> found_inf, bool nesterov,
-                    std::vector<bool> first, std::vector<int64_t> rows, at::Tensor stats, double trust, double eps, bool clip) {
+                    std::vector<bool> first, std::vector<int64_t> rows, at::Tensor stats, double trust, double eps, bool clip,
+                    std::vector<at::Tensor> ema) {
   const size_t n = params.size();
   if (n == 0) return;
   TORCH_CHECK(grads.size() == n && momenta.size() == n && first.size() == n && rows.size() == n, "LARC lists must have one entry per tensor");
@@ -594,6 +707,7 @@ void larc_sgd_multi(std::vector<at::Tensor> grads, std::vector<at::Tensor> param
   for (auto& p : params) TORCH_CHECK(p.scalar_type() == at::kFloat, "params (masters) must be fp32");
   for (auto& m : momenta) TORCH_CHECK(m.scalar_type() == at::kFloat, "momentum must be fp32");
   check_larc_common(hyper, found_inf, stats, trust, eps);
+  check_ema_multi(ema, params, hyper);
   std::vector<at::Tensor> copies;
   for (auto& c : model_copies) copies.push_back(c.has_value() ? *c : at::Tensor());
   std::vector<int32_t> cbase(n);
@@ -624,9 +738,17 @@ void larc_sgd_multi(std::vector<at::Tensor> grads, std::vector<at::Tensor> param
     larc_norm_multi_kernel<<<nb, kLarcThreads, 0, st>>>(a, slots(src, a.block_tensor[nb - 1] + 1), part, hp, fi);
     C10_CUDA_KERNEL_LAUNCH_CHECK();
   });
+  if (!ema.empty()) {
+    mta_for_each<5>({grads, params, momenta, copies, ema}, [&](const MtaArgs<5>& a, int nb, const int* src) {
+      larc_sgd_multi_kernel<true><<<nb, kLarcThreads, 0, st>>>(a, slots(src, a.block_tensor[nb - 1] + 1), part, stats.data_ptr<float>(), hp, fi,
+                                                               nesterov, (float)trust, (float)eps, clip);
+      C10_CUDA_KERNEL_LAUNCH_CHECK();
+    });
+    return;
+  }
   mta_for_each<4>({grads, params, momenta, copies}, [&](const MtaArgs<4>& a, int nb, const int* src) {
-    larc_sgd_multi_kernel<<<nb, kLarcThreads, 0, st>>>(a, slots(src, a.block_tensor[nb - 1] + 1), part, stats.data_ptr<float>(), hp, fi,
-                                                       nesterov, (float)trust, (float)eps, clip);
+    larc_sgd_multi_kernel<false><<<nb, kLarcThreads, 0, st>>>(a, slots(src, a.block_tensor[nb - 1] + 1), part, stats.data_ptr<float>(), hp, fi,
+                                                              nesterov, (float)trust, (float)eps, clip);
     C10_CUDA_KERNEL_LAUNCH_CHECK();
   });
 }

@@ -29,7 +29,7 @@ import torch.nn as nn
 
 from . import cli
 from .models import create_model
-from .utils.checkpoint import export_state_dict, load_checkpoint, save_checkpoint
+from .utils.checkpoint import export_ema_state_dict, export_state_dict, load_checkpoint, save_checkpoint
 from .utils.data import DataPrefetcher, build_loaders
 from .utils.meters import AverageMeter, ProgressMeter, accuracy, adjust_learning_rate
 
@@ -203,8 +203,9 @@ class TrainStep:
     graphs, one memory pool).
     """
 
-    def __init__(self, st, model, criterion, optimizer, metrics, use_graph: bool = False, warmup: int = 3):
+    def __init__(self, st, model, criterion, optimizer, metrics, use_graph: bool = False, warmup: int = 3, ema=None):
         self.st, self.model, self.criterion, self.optimizer, self.metrics = st, model, criterion, optimizer, metrics
+        self.ema = ema if ema is not None else getattr(st, "model_ema", None)   # --model-ema: once per optimizer step
         self.use_graph = bool(use_graph) and torch.cuda.is_available()
         self.warmup = warmup
         self.calls = 0
@@ -248,6 +249,8 @@ class TrainStep:
             torch.cuda.nvtx.range_pop()
             torch.cuda.nvtx.range_push("ptd.optimizer")
         self.optimizer.step()
+        if self.ema is not None:
+            self.ema.update()           # a fused optimizer has already averaged inside its step: no-op then
         if nvtx:
             torch.cuda.nvtx.range_pop()
         self.metrics.join()
@@ -405,6 +408,12 @@ class Strategy:
         return model
 
     def build(self, model, args, device, local_rank):
+        """Precision, wrapper and optimizer (``build_model``), then the ``--model-ema`` average of the finished model."""
+        model, optimizer = self.build_model(model, args, device, local_rank)
+        self.model_ema = make_model_ema(model, optimizer, args)
+        return model, optimizer
+
+    def build_model(self, model, args, device, local_rank):
         model = self.prepare_model(model, args, device)
         model = self.wrap(model, args, device, local_rank)
         optimizer = self.make_optimizer(model, args)
@@ -433,7 +442,7 @@ class ApexStrategy(Strategy):
     name = "apex_distributed"
     raw_uint8_loader = False
 
-    def build(self, model, args, device, local_rank):
+    def build_model(self, model, args, device, local_rank):
         from .apex import amp
         from .apex.parallel import DistributedDataParallel as ApexDDP
         model.to(device)
@@ -487,7 +496,7 @@ class HorovodStrategy(Strategy):
     def rank(self):
         return self.hvd.rank()
 
-    def build(self, model, args, device, local_rank):
+    def build_model(self, model, args, device, local_rank):
         hvd = self.hvd
         model = self.prepare_model(model, args, device)
         hvd.broadcast_parameters(model.state_dict(), root_rank=0)
@@ -526,7 +535,7 @@ class DataParallelStrategy(Strategy):
     def init_process_group(self, args, local_rank, nprocs):
         pass
 
-    def build(self, model, args, device, local_rank):
+    def build_model(self, model, args, device, local_rank):
         from .parallel.dp import DataParallel
         if args.gpus:
             gpus = [int(g) for g in args.gpus.split(",")]
@@ -606,9 +615,19 @@ def main_worker(local_rank: int, nprocs: int, args, strategy: Optional[Strategy]
         args.start_epoch = ck.get("epoch", args.start_epoch)
         best_acc1 = float(ck.get("best_acc1", 0.0))
         print("=> loaded checkpoint '{}' (epoch {})".format(args.resume, args.start_epoch))
+    ema = getattr(st, "model_ema", None)
+    if ema is not None and args.resume:
+        if ck.get("state_dict_ema") is not None:
+            ema.load_state_dict(ck["state_dict_ema"])
+        else:
+            ema.reset()
+            if not st.distributed or st.rank() == 0:
+                print("=> no state_dict_ema in checkpoint '{}': the EMA starts from the resumed weights".format(args.resume))
 
     if args.evaluate:
         validate(val_loader, model, criterion, st, device, args)
+        if ema is not None:
+            validate_ema(ema, val_loader, criterion, st, device, args)
         _shutdown(st)
         return
 
@@ -619,21 +638,40 @@ def main_worker(local_rank: int, nprocs: int, args, strategy: Optional[Strategy]
         adjust_learning_rate(optimizer, epoch, args)
         train(train_loader, model, criterion, optimizer, epoch, st, device, args)
         acc1 = validate(val_loader, model, criterion, st, device, args)
-        is_best = acc1 > best_acc1
+        if ema is not None:
+            validate_ema(ema, val_loader, criterion, st, device, args)
+        is_best = acc1 > best_acc1          # model_best follows the live model's Acc@1
         best_acc1 = max(acc1, best_acc1)
         if st.epoch_csv and st.is_saver(args):
             with open(os.path.join(args.checkpoint_dir, st.epoch_csv), "a+", newline="") as f:
                 csv.writer(f).writerow([time.strftime("%Y-%m-%d %H:%M:%S", time.localtime(t_epoch)), time.time() - t_epoch])
         if st.is_saver(args):
-            save_checkpoint({
+            state = {
                 "epoch": epoch + 1,
                 "arch": args.arch,
                 "state_dict": export_state_dict(st.unwrapped(model), getattr(st, "engine", None), optimizer),
                 "best_acc1": best_acc1,
                 "optimizer": optimizer.state_dict() if args.resume or os.environ.get("PTD_SAVE_OPTIMIZER") else None,
                 "amp": st.amp.state_dict() if hasattr(st, "amp") else None,      # loss-scaler state (apex entrypoint)
-            }, is_best, directory=args.checkpoint_dir)
+            }
+            if ema is not None:
+                state["state_dict_ema"] = export_ema_state_dict(ema)
+            save_checkpoint(state, is_best, directory=args.checkpoint_dir)
     _shutdown(st)
+
+
+def make_model_ema(model, optimizer, args):
+    """``--model-ema``: the ModelEma of the unwrapped model, attached to the optimizer (None without the flag)."""
+    if not getattr(args, "model_ema", False):
+        return None
+    from .utils.ema import ModelEma
+    return ModelEma(model, decay=args.model_ema_decay, optimizer=optimizer)
+
+
+def validate_ema(ema, val_loader, criterion, st, device, args):
+    """Validate the averaged weights: ``ema.module`` (DataParallel: on its first device alone, without replicas)."""
+    ema.sync_module()
+    return validate(val_loader, ema.module, criterion, st, device, args, tag="EMA")
 
 
 class _DeviceStepTimer:
@@ -777,14 +815,15 @@ def train(train_loader, model, criterion, optimizer, epoch, st: Strategy, device
     return losses.avg
 
 
-def validate(val_loader, model, criterion, st: Strategy, device, args):
-    """/root/reference/distributed.py:279-324 - distributed evaluation: sharded val set + metric all-reduce."""
+def validate(val_loader, model, criterion, st: Strategy, device, args, tag: Optional[str] = None):
+    """/root/reference/distributed.py:279-324 - distributed evaluation: sharded val set + metric all-reduce.
+    ``tag="EMA"`` (``--model-ema``): the summary line reads `` * EMA Acc@1 ...`` and the JSONL phase ``val_ema``."""
     batch_time = AverageMeter("Time", ":6.3f")
     losses = AverageMeter("Loss", ":.4e")
     top1 = AverageMeter("Acc@1", ":6.2f")
     top5 = AverageMeter("Acc@5", ":6.2f")
     pf = st.prefetcher(val_loader, device, args, limit=args.val_steps or args.steps_per_epoch)
-    progress = ProgressMeter(len(pf), [batch_time, losses, top1, top5], prefix="Test: ")
+    progress = ProgressMeter(len(pf), [batch_time, losses, top1, top5], prefix="Test: " if tag is None else "Test %s: " % tag)
     metrics = MetricPipeline(getattr(st, "comm", None), device, (losses, top1, top5), reduce=st.reduce_metrics)
     model.eval()
     with torch.no_grad():
@@ -802,6 +841,7 @@ def validate(val_loader, model, criterion, st: Strategy, device, args):
                     progress.display(i)
         metrics.drain()
         # printed by every rank, like the reference (/root/reference/distributed.py:320-321)
-        print(" * Acc@1 {top1.avg:.3f} Acc@5 {top5.avg:.3f}".format(top1=top1, top5=top5), flush=True)
-    _log_jsonl(args, {"phase": "val", "rank": st.rank() if st.distributed else 0, "loss": losses.avg, "acc1": top1.avg, "acc5": top5.avg})
+        print(" *{tag} Acc@1 {top1.avg:.3f} Acc@5 {top5.avg:.3f}".format(tag="" if tag is None else " " + tag, top1=top1, top5=top5),
+              flush=True)
+    _log_jsonl(args, {"phase": "val" if tag is None else "val_" + tag.lower(), "rank": st.rank() if st.distributed else 0, "loss": losses.avg, "acc1": top1.avg, "acc5": top5.avg})
     return top1.avg

@@ -12,6 +12,10 @@ Three execution modes, picked automatically:
 
 ``enable_larc`` (what ``apex.parallel.LARC`` calls) adds layer-wise adaptive rates to all three modes: a norm pass and an
 update pass per flat step, per bucket in overlap mode, or per group in multi-tensor mode (``csrc/optim.cu``).
+
+``attach_ema`` (what :class:`~pytorch_distributed_b200.utils.ema.ModelEma` calls) folds an exponential moving average of
+the fp32 masters into the update kernels of every mode (one more fp32 read and write per element), and averages the
+model's float buffers with one ``ema_multi`` launch at the end of each step.  The decay sits in hyper slots 6 and 7.
 """
 from __future__ import annotations
 
@@ -76,6 +80,8 @@ class FusedSGD(Optimizer):
         self._larc = None           # (trust_coefficient, clip, eps) in LARC mode (enable_larc)
         self._larc_stats = None     # [n_params, 3] fp32 {pn, gn, f} of the last applied step
         self._larc_tab = None       # flat mode: chunk table of the arena layout (built once)
+        self._ema = None            # ModelEma updated inside the step (attach_ema)
+        self._ema_flat = None       # flat mode: its parameter averages in the arena layout
         self._try_bind()
 
     # ------------------------------------------------------------------ engine binding (flat mode)
@@ -95,7 +101,10 @@ class FusedSGD(Optimizer):
         self._flat = eng.bind_flat_optimizer(self, params)
         if self._flat is None:
             self._bind_refused = True
-        elif self._overlap and getattr(eng, "supports_overlap_optimizer", False):
+            return
+        if self._ema is not None:
+            self._ema_to_flat()
+        if self._overlap and getattr(eng, "supports_overlap_optimizer", False):
             eng.set_overlap_optimizer(self)
 
     # ------------------------------------------------------------------ overlap mode (called by the gradient engine)
@@ -126,8 +135,9 @@ class FusedSGD(Optimizer):
             return
         _ext.note_launch()
         copy = fs.model_copy[off:off + n] if fs.model_copy is not None else None
+        ema = self._ema_flat[off:off + n] if self._ema_flat is not None else None
         _ext.lib().fused_sgd_flat(fs.engine.grad_arena()[off:off + n], fs.master[off:off + n], fs.momentum[off:off + n], copy,
-                                  self._hyper[0][0], None, bool(self.param_groups[0]["nesterov"]), self._ov_first)
+                                  self._hyper[0][0], None, bool(self.param_groups[0]["nesterov"]), self._ov_first, ema=ema)
         self._ov_applied += n
 
     # ------------------------------------------------------------------ LARC (apex.parallel.LARC semantics)
@@ -201,7 +211,45 @@ class FusedSGD(Optimizer):
         _ext.note_launch(2)
         _ext.lib().larc_sgd_flat(fs.engine.grad_arena(), fs.master, fs.momentum, fs.model_copy, hyper, found_inf,
                                  bool(self.param_groups[0]["nesterov"]), first, tab.chunk_tensor, tab.info, lo, hi, tab.partials,
-                                 self._larc_stats_on(fs.master.device), trust, eps, clip)
+                                 self._larc_stats_on(fs.master.device), trust, eps, clip, ema=self._ema_flat)
+
+    # ------------------------------------------------------------------ exponential moving average (ModelEma)
+    def attach_ema(self, ema) -> None:
+        """Update ``ema`` (a :class:`~pytorch_distributed_b200.utils.ema.ModelEma` over this optimizer's model) inside every
+        applied step: its parameter averages in the update kernels, its float buffers right after them."""
+        self._ema = ema
+        if self._flat is not None:
+            self._ema_to_flat()
+        self.refresh_hyper()
+
+    def _ema_to_flat(self):
+        """Move the parameter averages into one fp32 buffer with the arena layout (the flat kernels stream it next to the
+        masters); the average's tensors become views of it.  The padding between tensors follows the masters."""
+        fs, ema = self._flat, self._ema
+        eng = fs.engine
+        flat = fs.master.clone()
+        with torch.no_grad():
+            for pid, p in enumerate(eng.params):
+                off, cnt = eng.param_elem_off[pid], p.numel()
+                view = flat[off:off + cnt].as_strided(p.size(), p.stride())
+                view.copy_(ema.shadow_of(p))
+                ema.set_shadow_of(p, view)
+        self._ema_flat = flat
+
+    def _ema_multi_lists(self, params):
+        return [self._ema.shadow_of(p) for p in params] if self._ema is not None else []
+
+    def _ema_buffers(self, hyper, found_inf, pairs=None):
+        """Average the model's float buffers (BatchNorm running statistics) with the decay in ``hyper[6:8]``; skipped
+        with the step when ``found_inf`` is set."""
+        if self._ema is None:
+            return
+        live, shadow = pairs if pairs is not None else self._ema.buffer_pairs()
+        if not live:
+            return
+        from .. import _ext
+        _ext.note_launch()
+        _ext.lib().ema_multi(live, shadow, hyper[6:8], found_inf)
 
     @property
     def is_flat(self) -> bool:
@@ -211,18 +259,22 @@ class FusedSGD(Optimizer):
     def _hyper_tensor(self, gi: int, group, device):
         gmul = 1.0
         vals = (float(group["lr"]), float(group["momentum"]), float(group["weight_decay"]), float(group["dampening"]))
+        dw = self._ema.decay_pair() if self._ema is not None else (0.0, 0.0)      # slots 6, 7: EMA decay d and fp32(1 - d)
         ent = self._hyper.get(gi)
         if ent is None:
             # slot 5 (momentum_pending): under dynamic loss scaling the momentum is initialised by the first step that is
             # actually applied; the loss scaler clears the slot after it (csrc/optim.cu)
             pending = 1.0 if self._steps == 0 else 0.0
-            t = torch.tensor(list(vals) + [gmul, pending, 0, 0], dtype=torch.float32, device=device)
-            self._hyper[gi] = [t, vals]
+            t = torch.tensor(list(vals) + [gmul, pending] + list(dw), dtype=torch.float32, device=device)
+            self._hyper[gi] = [t, vals, dw]
             return t
         if ent[1] != vals:
-            # only lr..dampening are host-owned; slot 4 (gradient multiplier) belongs to the loss scaler kernel
+            # only lr..dampening and the EMA slots are host-owned; slot 4 (gradient multiplier) belongs to the loss scaler kernel
             ent[0][:4].copy_(torch.tensor(vals, dtype=torch.float32), non_blocking=True)
             ent[1] = vals
+        if ent[2] != dw:
+            ent[0][6:8].copy_(torch.tensor(dw, dtype=torch.float32), non_blocking=True)
+            ent[2] = dw
         return ent[0]
 
     def refresh_hyper(self) -> None:
@@ -249,7 +301,8 @@ class FusedSGD(Optimizer):
             fs.engine.wait_for_gradients()
             group = self.param_groups[0]
             if self._ov_active and self._ov_applied == fs.master.numel():
-                self._ov_applied = 0       # every bucket was updated behind its all-reduce during backward: nothing left to do
+                self._ov_applied = 0       # every bucket was updated behind its all-reduce during backward: only the buffers
+                self._ema_buffers(self._hyper[0][0], None)
                 self._steps += 1
                 return loss
             if self._ov_applied:
@@ -264,12 +317,15 @@ class FusedSGD(Optimizer):
             else:
                 _ext.note_launch()
                 _ext.lib().fused_sgd_flat(fs.engine.grad_arena(), fs.master, fs.momentum, fs.model_copy, hyper,
-                                          amp.found_inf if amp is not None else None, bool(group["nesterov"]), first)
+                                          amp.found_inf if amp is not None else None, bool(group["nesterov"]), first,
+                                          ema=self._ema_flat)
+            self._ema_buffers(hyper, amp.found_inf if amp is not None else None)
             if amp is not None:
                 amp.update()
         else:
             for gi, group in enumerate(self.param_groups):
                 self._step_group(gi, group, first, amp)
+            self._ema_buffers_multi(amp)
             if amp is not None:
                 amp.update()
         self._steps += 1
@@ -329,7 +385,7 @@ class FusedSGD(Optimizer):
                                  [None if p.dtype == torch.float32 else p.data for p in params], hyper,
                                  amp.found_inf if amp is not None else None, bool(group["nesterov"]),
                                  [id(p) in fresh_ids for p in params], [rows[id(p)] for p in params],
-                                 self._larc_stats_on(params[0].device), trust, eps, clip)
+                                 self._larc_stats_on(params[0].device), trust, eps, clip, ema=self._ema_multi_lists(params))
                 return
             fs = set(fresh) if (fresh and len(fresh) != len(params)) else None      # rare: first gradient later than the others
             for first_flag, sub in ((True, fresh), (False, [p for p in params if p not in fs])) if fs is not None else ((bool(fresh), params),):
@@ -337,11 +393,12 @@ class FusedSGD(Optimizer):
                 low = [p for p in sub if p.dtype != torch.float32]
                 if full:
                     C.fused_sgd_multi([p.grad for p in full], full, [self.state[p]["momentum_buffer"] for p in full], [], hyper,
-                                      amp.found_inf if amp is not None else None, bool(group["nesterov"]), first_flag)
+                                      amp.found_inf if amp is not None else None, bool(group["nesterov"]), first_flag,
+                                      ema=self._ema_multi_lists(full))
                 if low:
                     C.fused_sgd_multi([p.grad for p in low], [master_of(p) for p in low], [self.state[p]["momentum_buffer"] for p in low],
                                       [p.data for p in low], hyper, amp.found_inf if amp is not None else None, bool(group["nesterov"]),
-                                      first_flag)
+                                      first_flag, ema=self._ema_multi_lists(low))
         else:
             if amp is not None and amp.host_found_inf():
                 return
@@ -363,6 +420,25 @@ class FusedSGD(Optimizer):
                 sgd_reference_step(master, g, buf, group["lr"], group["momentum"], wd, group["dampening"], group["nesterov"], fresh)
                 if master is not p:
                     p.copy_(master)
+                if self._ema is not None:
+                    from ..utils.ema import ema_reference_
+                    ema_reference_(self._ema.shadow_of(p), master, *self._ema.decay_pair())
+
+    def _ema_buffers_multi(self, amp):
+        """Buffer average after a multi-tensor or CPU step (the CPU path skips an overflowed step on the host)."""
+        if self._ema is None:
+            return
+        live, shadow = self._ema.buffer_pairs()
+        if not live:
+            return
+        if live[0].is_cuda:
+            dev = live[0].device
+            self._ema_buffers(self._hyper_tensor(0, self.param_groups[0], dev), amp.found_inf if amp is not None else None,
+                              (live, shadow))
+        elif amp is None or not amp.host_found_inf():
+            from ..utils.ema import ema_reference_
+            for b, e in zip(live, shadow):
+                ema_reference_(e, b, *self._ema.decay_pair())
 
     def zero_grad(self, set_to_none: bool = True):
         super().zero_grad(set_to_none=set_to_none)

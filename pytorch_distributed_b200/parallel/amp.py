@@ -146,6 +146,7 @@ def _wrap_forward(model: nn.Module, autocast_dtype: Optional[torch.dtype], input
                 return inner(*args, **kwargs)
         return inner(*args, **kwargs)
 
+    forward._ptd_amp = (autocast_dtype, input_dtype)        # lets a copy of the model (ModelEma) be wrapped the same way
     model.forward = forward
     return model
 
@@ -195,7 +196,9 @@ def _patch_stock_optimizer(opt, scaler: LossScaler):
     inner = opt.step
 
     def step(*a, **kw):
-        if getattr(opt, "_amp_skip", False):
+        skip = bool(getattr(opt, "_amp_skip", False))
+        opt._amp_last_skipped = skip            # read by ModelEma.update(): a skipped step is not averaged either
+        if skip:
             opt._amp_skip = False
             return None
         return inner(*a, **kw)

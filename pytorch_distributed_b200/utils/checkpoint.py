@@ -4,7 +4,8 @@ Reference: ``save_checkpoint`` /root/reference/distributed.py:327-330 and its ca
 ``checkpoint.pth.tar`` / ``model_best.pth.tar`` in the working directory, keys ``epoch`` (= epoch + 1), ``arch``,
 ``state_dict`` (the *unwrapped* module), ``best_acc1``.  The state dict written here is always fp32, whatever
 precision the arenas / model copy run in.  ``--resume`` (SURVEY Q10) is an additive extension; optimizer and
-loss-scaler state ride along under extra keys that a reference-style reader simply ignores.
+loss-scaler state ride along under extra keys that a reference-style reader simply ignores, and so does
+``state_dict_ema`` (``--model-ema``: the fp32 weight averages under the unwrapped module's keys).
 """
 from __future__ import annotations
 
@@ -40,6 +41,12 @@ def export_state_dict(module: torch.nn.Module, engine=None, optimizer=None):
             v = v.cpu().contiguous().clone()
         out[k] = v
     return out
+
+
+def export_ema_state_dict(ema):
+    """``state_dict_ema``: fp32 CPU copy of :meth:`ModelEma.state_dict` (loads into a fresh model of the architecture)."""
+    sd = ema.state_dict()
+    return type(sd)((k, v.detach().cpu().contiguous() if torch.is_tensor(v) else v) for k, v in sd.items())
 
 
 def save_checkpoint(state, is_best: bool, filename: str = "checkpoint.pth.tar", directory: str = ".") -> str:

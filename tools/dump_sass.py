@@ -19,7 +19,7 @@ WANT = {
     "push_bf16_nvls": r"push_kernelI13__nv_bfloat16Lb1E",
     "metrics_bf16": r"metrics_kernelI13__nv_bfloat16E",
     "barrier": r"barrier_kernel",
-    "fused_sgd_flat_bf16": r"fused_sgd_flat_kernelI13__nv_bfloat16S1_Lb1E",
+    "fused_sgd_flat_bf16": r"fused_sgd_flat_kernelI13__nv_bfloat16S1_Lb1ELb0E",
     "gemm_bnstats_wgmma_n256": r"gemm_bnstats_kernelILi256E",
     "gemm_bnstats_wgmma_n64": r"gemm_bnstats_kernelILi64E",
     "combine_partials": r"combine_partials_kernel",

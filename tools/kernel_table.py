@@ -21,8 +21,12 @@ KERNELS = [
     (r"metrics_kernelI13__nv_bfloat16E", "metrics_kernel<bf16>", "collectives.cu", "K4: top-1/top-5 counting + LL all-reduce of {loss, acc1, acc5}", "tests/test_gpu_kernels.py"),
     (r"ll_allreduce_kernel", "ll_allreduce_kernel", "collectives.cu", "<= 8 scalars, flag-in-payload protocol", "tests/mp_gpu_checks.py"),
     (r"barrier_kernel", "barrier_kernel", "collectives.cu", "K3", "tests/mp_gpu_checks.py"),
-    (r"fused_sgd_flat_kernelI13__nv_bfloat16S1_Lb1E", "fused_sgd_flat_kernel<bf16 grad, bf16 model>", "optim.cu",
+    (r"fused_sgd_flat_kernelI13__nv_bfloat16S1_Lb1ELb0E", "fused_sgd_flat_kernel<bf16 grad, bf16 model>", "optim.cu",
      "K6: unscale + overflow skip + SGD momentum over arena / fp32 masters / momentum / bf16 copy", "tests/test_gpu_kernels.py"),
+    (r"fused_sgd_flat_kernelI13__nv_bfloat16S1_Lb1ELb1E", "fused_sgd_flat_kernel<bf16 grad, bf16 model, EMA>", "optim.cu",
+     "K6 + --model-ema epilogue: fp32 weight average e = fmaf(d, e, w p) from the new masters", "tests/test_gpu_model_ema.py, tools/ema_bench.py"),
+    (r"ema_multi_kernel", "ema_multi_kernel", "optim.cu", "--model-ema: BN buffers / stock-optimizer weights averaged, multi-tensor",
+     "tests/test_gpu_model_ema.py, tools/ema_bench.py"),
     (r"grad_accumulate_kernel", "grad_accumulate_kernel", "collectives.cu",
      "--accum-steps: bucket gradients added into the rank-local fp32 sum (no_sync passes)", "tests/test_gpu_grad_accum.py, tools/accum_bench.py"),
     (r"grad_fold_kernel", "grad_fold_kernel", "collectives.cu",
@@ -30,7 +34,7 @@ KERNELS = [
     (r"fused_sgd_multi_kernel", "fused_sgd_multi_kernel", "optim.cu", "multi-tensor-apply variant (non-flat parameters)", "tests/test_gpu_kernels.py"),
     (r"larc_norm_flat_kernelI13__nv_bfloat16E", "larc_norm_flat_kernel<bf16>", "optim.cu",
      "LARC norm pass: per-chunk fp32 sums of p^2 and (g gmul)^2 over the arena, fixed order", "tests/test_gpu_larc.py, tools/larc_bench.py"),
-    (r"larc_sgd_flat_kernelI13__nv_bfloat16S1_Lb1E", "larc_sgd_flat_kernel<bf16 grad, bf16 model>", "optim.cu",
+    (r"larc_sgd_flat_kernelI13__nv_bfloat16S1_Lb1ELb0E", "larc_sgd_flat_kernel<bf16 grad, bf16 model>", "optim.cu",
      "LARC update: trust ratio from the chunk partials + SGD momentum + bf16 copy + statistics", "tests/test_gpu_larc.py, tools/larc_bench.py"),
     (r"larc_norm_multi_kernel", "larc_norm_multi_kernel", "optim.cu", "LARC norm pass, multi-tensor-apply variant", "tests/test_gpu_larc.py"),
     (r"larc_sgd_multi_kernel", "larc_sgd_multi_kernel", "optim.cu", "LARC update, multi-tensor-apply variant", "tests/test_gpu_larc.py"),
