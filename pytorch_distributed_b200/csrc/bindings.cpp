@@ -148,6 +148,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         sync_arg);
   m.def("stem_im2col", &stem_im2col);
   m.def("conv1x1_bnstats", &conv1x1_bnstats, py::arg("x"), py::arg("weight"), py::arg("gsum"), sync_arg);
+  m.def("conv1x1_bn_backward", &conv1x1_bn_backward, py::arg("dy_a"), py::arg("dy_b"), py::arg("y"), py::arg("mask"), py::arg("weight"),
+        py::arg("saved"), py::arg("conv_weight"), py::arg("relu"), py::arg("work"));
   m.def("normalize_nhwc", &normalize_nhwc);
   m.def("resample_normalize", &resample_normalize, py::arg("arena"), py::arg("n"), py::arg("out_h"), py::arg("out_w"), py::arg("max_rows"),
         py::arg("a"), py::arg("b"), py::arg("out_dtype"), py::arg("channels_last"));

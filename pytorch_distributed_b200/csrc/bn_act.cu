@@ -48,21 +48,6 @@ __device__ __forceinline__ RowMap row_map(int C) {
   return m;
 }
 
-__device__ __forceinline__ float ld_w(const void* p, int dt, int i) {
-  switch (dt) {
-    case kF32: return reinterpret_cast<const float*>(p)[i];
-    case kBF16: return __bfloat162float(reinterpret_cast<const __nv_bfloat16*>(p)[i]);
-    default: return __half2float(reinterpret_cast<const __half*>(p)[i]);
-  }
-}
-__device__ __forceinline__ void st_w(void* p, int dt, int i, float v) {
-  switch (dt) {
-    case kF32: reinterpret_cast<float*>(p)[i] = v; break;
-    case kBF16: reinterpret_cast<__nv_bfloat16*>(p)[i] = __float2bfloat16_rn(v); break;
-    default: reinterpret_cast<__half*>(p)[i] = __float2half_rn(v); break;
-  }
-}
-
 // Combine the per-thread partial sums (a[8], b[8] for channel group `cg`) of a CTA into this CTA's row of the partials,
 // part[blockIdx.x][0:C] / [C:2C]; combine_partials() then adds the rows in a fixed order.
 // Caller loops over channel-group chunks; `sm` holds [slots][2 * tpr * 8] floats.
@@ -338,11 +323,9 @@ __device__ __forceinline__ void bn_bwd_apply_body(BN_BWD_APPLY_PARAMS) {
 #pragma unroll
     for (int k = 0; k < 8; ++k) {
       const int c = cg * 8 + k;
-      const float mean = saved[c], invstd = saved[C + c];
       const float sdz = gsum[c], sdzx = gsum[C + c];
-      ka[k] = ld_w(w, wdt, c) * invstd;
-      kb[k] = -ka[k] * invstd * sdzx * inv_m;
-      kd[k] = -ka[k] * sdz * inv_m - kb[k] * mean;
+      const BnBwdCoef q = bn_bwd_coef(ld_w(w, wdt, c), saved[c], saved[C + c], sdz, sdzx, inv_m, SYNC || k == 7);
+      ka[k] = q.a; kb[k] = q.b; kd[k] = q.d;
       if (blockIdx.x == 0 && m.rlocal == 0) {
         if constexpr (SYNC) {
           st_w(dw, wdt, c, gsum[c - C]);          // local sum dz * xhat
@@ -374,7 +357,7 @@ __device__ __forceinline__ void bn_bwd_apply_body(BN_BWD_APPLY_PARAMS) {
           float dz = d[u][k];
           if constexpr (RELU) dz = (bits[u] >> k) & 1u ? dz : 0.f;
           d[u][k] = dz;
-          v[u][k] = ka[k] * dz + kb[k] * v[u][k] + kd[k];
+          v[u][k] = bn_bwd_dx(ka[k], kb[k], kd[k], dz, v[u][k]);
         }
         store8<T>(dx + off, v[u]);
         if constexpr (RES) store8<T>(dres + off, d[u]);
@@ -392,7 +375,7 @@ __device__ __forceinline__ void bn_bwd_apply_body(BN_BWD_APPLY_PARAMS) {
         float dz = d[k];
         if constexpr (RELU) dz = (bits >> k) & 1u ? dz : 0.f;
         d[k] = dz;
-        v[k] = ka[k] * dz + kb[k] * v[k] + kd[k];
+        v[k] = bn_bwd_dx(ka[k], kb[k], kd[k], dz, v[k]);
       }
       store8<T>(dx + off, v);
       if constexpr (RES) store8<T>(dres + off, d);
@@ -575,6 +558,19 @@ static void bwd_apply(const Geometry& g, const at::Tensor& part, const T* dy, co
   C10_CUDA_KERNEL_LAUNCH_CHECK();
 }
 
+// First pass of a BatchNorm backward: the per-CTA partials of sum dz and sum dz * xhat, dz = dy (x the ReLU bits with `mask`)
+template <typename T>
+static at::Tensor bwd_reduce(const Geometry& g, const T* dy, const uint8_t* mask, const at::Tensor& x, const at::Tensor& saved, cudaStream_t st) {
+  const auto reduce = mask ? bn_bwd_reduce_kernel<T, true> : bn_bwd_reduce_kernel<T, false>;
+  int rpb;
+  const int rgrid = reduce_grid(g, &rpb, resident_ctas(reduce, g.smem));
+  at::Tensor part = partials(x, rgrid, g.C);
+  reduce<<<rgrid, kBnThreads, g.smem, st>>>(dy, mask, reinterpret_cast<const T*>(x.data_ptr()), saved.data_ptr<float>(), part.data_ptr<float>(),
+                                            g.M, g.C, rpb);
+  C10_CUDA_KERNEL_LAUNCH_CHECK();
+  return part;
+}
+
 template <typename T>
 static void bwd_impl(const at::Tensor& dy, const at::Tensor& mask, const at::Tensor& x, const at::Tensor& saved, at::Tensor& work,
                      const at::Tensor& w, at::Tensor& dx, at::Tensor& dres, at::Tensor& dw, at::Tensor& db, bool relu, bool write_res,
@@ -583,13 +579,7 @@ static void bwd_impl(const at::Tensor& dy, const at::Tensor& mask, const at::Ten
   cudaStream_t st = at::cuda::getCurrentCUDAStream();
   const T* dyp = reinterpret_cast<const T*>(dy.data_ptr());
   const uint8_t* mk = relu ? mask.data_ptr<uint8_t>() : nullptr;
-  const auto reduce = relu ? bn_bwd_reduce_kernel<T, true> : bn_bwd_reduce_kernel<T, false>;
-  int rpb;
-  const int rgrid = reduce_grid(g, &rpb, resident_ctas(reduce, g.smem));
-  at::Tensor part = partials(x, rgrid, g.C);
-  reduce<<<rgrid, kBnThreads, g.smem, st>>>(dyp, mk, reinterpret_cast<const T*>(x.data_ptr()), saved.data_ptr<float>(), part.data_ptr<float>(),
-                                            g.M, g.C, rpb);
-  C10_CUDA_KERNEL_LAUNCH_CHECK();
+  at::Tensor part = bwd_reduce<T>(g, dyp, mk, x, saved, st);
   bwd_apply<T>(g, part, dyp, mk, x, saved, work, w, dx, write_res ? reinterpret_cast<T*>(dres.data_ptr()) : nullptr, dw, db, relu, sync, st);
 }
 
@@ -691,6 +681,21 @@ __global__ void __launch_bounds__(kBnThreads) bn_bwd_reduce_sum_kernel(const T* 
   }
 }
 
+// First pass with a split incoming gradient: writes g = (dy_a + dy_b) (x the ReLU bits) and returns the per-CTA partials
+template <typename T>
+static at::Tensor bwd_reduce_sum(const Geometry& g, const at::Tensor& dya, const at::Tensor& dyb, const uint8_t* mask, const at::Tensor& x,
+                                 const at::Tensor& saved, T* gout, cudaStream_t st) {
+  const auto reduce = mask ? bn_bwd_reduce_sum_kernel<T, true> : bn_bwd_reduce_sum_kernel<T, false>;
+  int rpb;
+  const int rgrid = reduce_grid(g, &rpb, resident_ctas(reduce, g.smem));
+  at::Tensor part = partials(x, rgrid, g.C);
+  reduce<<<rgrid, kBnThreads, g.smem, st>>>(reinterpret_cast<const T*>(dya.data_ptr()), reinterpret_cast<const T*>(dyb.data_ptr()), mask,
+                                            reinterpret_cast<const T*>(x.data_ptr()), saved.data_ptr<float>(), gout, part.data_ptr<float>(),
+                                            g.M, g.C, rpb);
+  C10_CUDA_KERNEL_LAUNCH_CHECK();
+  return part;
+}
+
 template <typename T>
 static void bwd2_impl(const at::Tensor& dya, const at::Tensor& dyb, const at::Tensor& mask, const at::Tensor& x, const at::Tensor& saved,
                       at::Tensor& work, const at::Tensor& w, at::Tensor& g_out, at::Tensor& dx, at::Tensor& dw, at::Tensor& db, bool relu,
@@ -698,14 +703,7 @@ static void bwd2_impl(const at::Tensor& dya, const at::Tensor& dyb, const at::Te
   const Geometry g = geometry(x);
   cudaStream_t st = at::cuda::getCurrentCUDAStream();
   T* gp = reinterpret_cast<T*>(g_out.data_ptr());
-  const auto reduce = relu ? bn_bwd_reduce_sum_kernel<T, true> : bn_bwd_reduce_sum_kernel<T, false>;
-  int rpb;
-  const int rgrid = reduce_grid(g, &rpb, resident_ctas(reduce, g.smem));
-  at::Tensor part = partials(x, rgrid, g.C);
-  reduce<<<rgrid, kBnThreads, g.smem, st>>>(reinterpret_cast<const T*>(dya.data_ptr()), reinterpret_cast<const T*>(dyb.data_ptr()),
-                                            relu ? mask.data_ptr<uint8_t>() : nullptr, reinterpret_cast<const T*>(x.data_ptr()),
-                                            saved.data_ptr<float>(), gp, part.data_ptr<float>(), g.M, g.C, rpb);
-  C10_CUDA_KERNEL_LAUNCH_CHECK();
+  at::Tensor part = bwd_reduce_sum<T>(g, dya, dyb, relu ? mask.data_ptr<uint8_t>() : nullptr, x, saved, gp, st);
   // second pass: g already carries the mask, and it IS the residual gradient -> the plain (no ReLU, no dres) apply variant
   bwd_apply<T>(g, part, gp, nullptr, x, saved, work, w, dx, nullptr, dw, db, false, sync, st);
 }
@@ -735,6 +733,59 @@ std::vector<at::Tensor> bn_act_backward2(const at::Tensor& dy_a_in, const at::Te
   at::Tensor dw = at::empty_like(weight), db = at::empty_like(weight);
   for_act_dtype(x, [&](auto t) { bwd2_impl<typename decltype(t)::type>(dya, dyb, mask, x, saved, work, weight, g, dx, dw, db, relu, sync); });
   return {dx, g, dw, db};
+}
+
+// ------------------------------------------------------------------ 1x1 conv -> BatchNorm pair: backward with the fused data gradient
+// The reduction pass as in bn_act_backward (dy_b undefined) or bn_act_backward2, then the wgmma data-gradient GEMM that forms
+// dx from g and y in shared memory as it loads them (gemm_bnstats.cu), instead of the apply pass followed by cuDNN's dgrad.
+// y: the BatchNorm input (the conv output); conv_weight: [C_out, C_in, 1, 1]; this rank alone (no synchronised statistics).
+// returns {d conv input, dx (d conv output, for the weight gradient), g (the residual gradient with dy_b, else undefined),
+//          dweight, dbias}
+std::vector<at::Tensor> conv1x1_bn_backward(const at::Tensor& dy_a_in, const c10::optional<at::Tensor>& dy_b_in, const at::Tensor& y,
+                                            const c10::optional<at::Tensor>& mask_opt, const at::Tensor& weight, const at::Tensor& saved,
+                                            const at::Tensor& conv_weight, bool relu, at::Tensor work) {
+  check_nhwc(y, "y");
+  const auto cl = at::MemoryFormat::ChannelsLast;
+  TORCH_CHECK(y.scalar_type() == at::kBFloat16 || y.scalar_type() == at::kHalf, "conv1x1_bn_backward: bf16 or fp16 activations");
+  at::Tensor dya = dy_a_in.is_contiguous(cl) ? dy_a_in : dy_a_in.contiguous(cl);
+  TORCH_CHECK(dya.scalar_type() == y.scalar_type() && dya.sizes() == y.sizes() && dya.device() == y.device(), "dy_a must match y");
+  const bool split = dy_b_in.has_value() && dy_b_in->defined();
+  at::Tensor dyb;
+  if (split) {
+    dyb = dy_b_in->is_contiguous(cl) ? *dy_b_in : dy_b_in->contiguous(cl);
+    TORCH_CHECK(dyb.scalar_type() == y.scalar_type() && dyb.sizes() == y.sizes() && dyb.device() == y.device(), "dy_b must match y");
+  }
+  const uint8_t* mk = nullptr;
+  if (relu) {
+    TORCH_CHECK(mask_opt.has_value() && mask_opt->defined() && mask_opt->scalar_type() == at::kByte && mask_opt->numel() == y.numel() / 8,
+                "ReLU backward needs the forward's bit mask");
+    mk = mask_opt->data_ptr<uint8_t>();
+  }
+  const int C = (int)y.size(1);
+  check_work(work, C, nullptr);
+  TORCH_CHECK(saved.defined() && saved.scalar_type() == at::kFloat && saved.numel() >= 2 * C, "saved statistics missing");
+  c10::cuda::CUDAGuard guard(y.device());
+  cudaStream_t st = at::cuda::getCurrentCUDAStream();
+  const Geometry g = geometry(y);
+  at::Tensor gt;                                  // the apply's input: dy_a, or the masked sum of the two gradients
+  at::Tensor part;
+  for_act_dtype(y, [&](auto t) {
+    using T = typename decltype(t)::type;
+    if (split) {
+      gt = at::empty_like(y, y.options().memory_format(cl));
+      part = bwd_reduce_sum<T>(g, dya, dyb, mk, y, saved, reinterpret_cast<T*>(gt.data_ptr()), st);
+      mk = nullptr;                               // g already carries the mask
+    } else {
+      gt = dya;
+      part = bwd_reduce<T>(g, reinterpret_cast<const T*>(dya.data_ptr()), mk, y, saved, st);
+    }
+  });
+  const float* sums = finish_sums(part.data_ptr<float>(), (int)part.size(0), C, g.M, work.data_ptr<float>(), nullptr, st);
+  at::Tensor dx = at::empty_like(y, y.options().memory_format(cl));
+  at::Tensor din = at::empty({y.size(0), conv_weight.size(1), y.size(2), y.size(3)}, y.options().memory_format(cl));
+  at::Tensor dw = at::empty_like(weight), db = at::empty_like(weight);
+  conv1x1_dgrad_bn(gt, y, mk, saved, sums, weight, wdtype(weight), dw, db, conv_weight, dx, din);
+  return {din, dx, split ? gt : at::Tensor(), dw, db};
 }
 
 }  // namespace ptd

@@ -29,6 +29,7 @@
 #include <cuda.h>
 #include <torch/extension.h>
 
+#include "bn_combine.cuh"
 #include "common.cuh"
 #include "host.h"
 
@@ -260,6 +261,229 @@ __global__ void __launch_bounds__(kGemmThreads, 1) gemm_bnstats_kernel(const __g
   }
 }
 
+// ------------------------------------------------------------------ data gradient with the BatchNorm backward apply on the A side
+//   dx[M, K]  = A_k * dz + B_k * y + D_k   (dz = g, times the ReLU bit with RELU; rounded to T: bn_bwd_dx, the bits of bn_bwd_apply)
+//   dIn[M, N] = dx x W                     (W = [K = C_out, N = C_in], the conv weight as stored: wgmma's transposed-B mode)
+// The backward of a 1x1 conv -> BN pair otherwise writes dx in the BN apply pass and reads it back in the dgrad GEMM; here
+// each stage's g tile is turned into the dx tile in place in shared memory before the wgmma reads it.  dx still reaches
+// global memory once (the weight gradient needs it): the CTAs of n-tile 0 TMA-store the transformed tiles, the others
+// re-read g / y from L2 like the forward kernel's A tiles.  wgmma group n-1 stays in flight while stage n is transformed.
+constexpr int kCoefMaxK = 2048;            // A / B / D of up to 2048 channels in shared memory
+
+template <int BLOCK_N> struct DgradCfg {
+  static constexpr int kStages = BLOCK_N == 128 ? 3 : 4;
+  static constexpr int kTileBytes = kBlockM * kBlockK * 2;            // one g or y tile
+  static constexpr int kBBytes = BLOCK_N * kBlockK * 2;               // [BLOCK_N / 64] boxes of 64 k-rows x 64 n
+  static constexpr int kCBytes = kBlockM * BLOCK_N * 2;
+  static constexpr int kSmem = 1024 + kStages * (2 * kTileBytes + kBBytes) + kCBytes + 2 * kStages * 8 + 3 * kCoefMaxK * 4;
+};
+
+// K-major A as in gmma_desc; MN-major 128B-swizzled B: 64-wide n atoms 8 KB apart (LBO), 8-row k groups 1 KB apart (SBO)
+__device__ __forceinline__ uint64_t gmma_desc_mn(const void* smem_tile) {
+  const uint64_t addr = (uint64_t)(smem_u32(smem_tile) >> 4) & 0x3FFFull;
+  return addr | ((uint64_t)(8192 >> 4) << 16) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 62);
+}
+
+#define PTD_F8(i) "+f"(d[i]), "+f"(d[i + 1]), "+f"(d[i + 2]), "+f"(d[i + 3]), "+f"(d[i + 4]), "+f"(d[i + 5]), "+f"(d[i + 6]), "+f"(d[i + 7])
+// as PTD_WGMMA_N64 / N128 with the transpose bit of B set (B read N-major)
+#define PTD_WGMMA_T64(TY)                                                                                             \
+  asm volatile(                                                                                                       \
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"                                                              \
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32." TY "." TY " "                                                     \
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "                                       \
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 1;\n\t}" \
+      : PTD_F8(0), PTD_F8(8), PTD_F8(16), PTD_F8(24)                                                                  \
+      : "l"(adesc), "l"(bdesc), "r"(accumulate))
+#define PTD_WGMMA_T128(TY)                                                                                            \
+  asm volatile(                                                                                                       \
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"                                                              \
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32." TY "." TY " "                                                    \
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "                                       \
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "                              \
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "                              \
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 1;\n\t}" \
+      : PTD_F8(0), PTD_F8(8), PTD_F8(16), PTD_F8(24), PTD_F8(32), PTD_F8(40), PTD_F8(48), PTD_F8(56)                  \
+      : "l"(adesc), "l"(bdesc), "r"(accumulate))
+template <typename T> __device__ __forceinline__ void wgmma_t64(float* d, uint64_t adesc, uint64_t bdesc, int accumulate) {
+  if constexpr (std::is_same<T, __half>::value) PTD_WGMMA_T64("f16");
+  else PTD_WGMMA_T64("bf16");
+}
+template <typename T> __device__ __forceinline__ void wgmma_t128(float* d, uint64_t adesc, uint64_t bdesc, int accumulate) {
+  if constexpr (std::is_same<T, __half>::value) PTD_WGMMA_T128("f16");
+  else PTD_WGMMA_T128("bf16");
+}
+#undef PTD_WGMMA_T64
+#undef PTD_WGMMA_T128
+#undef PTD_F8
+
+template <typename T, int BLOCK_N, bool RELU>
+__global__ void __launch_bounds__(kGemmThreads, 1) gemm_bnbwd_dgrad_kernel(
+    const __grid_constant__ CUtensorMap tmap_g, const __grid_constant__ CUtensorMap tmap_y, const __grid_constant__ CUtensorMap tmap_w,
+    const __grid_constant__ CUtensorMap tmap_dx, const __grid_constant__ CUtensorMap tmap_c, const uint8_t* __restrict__ mask,
+    const float* __restrict__ saved, const float* __restrict__ gsum, const void* __restrict__ bnw, int wdt, void* __restrict__ dw,
+    void* __restrict__ db, int M, int K, int m_tiles, int n_tiles, int ctas_per_n) {
+  using Cfg = DgradCfg<BLOCK_N>;
+  static_assert(BLOCK_N == 64 || BLOCK_N == 128, "one wgmma per k16 step");
+  constexpr int kStages = Cfg::kStages;
+  constexpr int kBoxes = BLOCK_N / 64;
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+  uint8_t* smem_g = smem;                                            // [kStages][128 x 64] T: g, rewritten to dx in place
+  uint8_t* smem_y = smem_g + kStages * Cfg::kTileBytes;              // [kStages][128 x 64] T: the BN input y
+  uint8_t* smem_b = smem_y + kStages * Cfg::kTileBytes;              // [kStages][kBoxes][64 k x 64 n] T
+  uint8_t* smem_c = smem_b + kStages * Cfg::kBBytes;                 // [2 warpgroups][kBoxes][64 x 64] T
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem_c + Cfg::kCBytes);
+  uint64_t* empty_bar = full_bar + kStages;
+  float* coef = reinterpret_cast<float*>(empty_bar + kStages);       // [A | B | D][K]
+
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int n_tile = blockIdx.x % n_tiles;
+  const int m_first = blockIdx.x / n_tiles;
+  const int n0 = n_tile * BLOCK_N;
+  const int num_kb = K / kBlockK;
+  const bool store_dx = n_tile == 0;
+
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < kStages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], kConsumerThreads / 32); }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  __syncthreads();
+
+  if (warp == kConsumerThreads / 32) {
+    // ===== TMA producer
+    if (lane == 0) {
+      asm volatile("prefetch.tensormap [%0];" ::"l"(&tmap_g) : "memory");
+      asm volatile("prefetch.tensormap [%0];" ::"l"(&tmap_y) : "memory");
+      asm volatile("prefetch.tensormap [%0];" ::"l"(&tmap_w) : "memory");
+      uint32_t it = 0;
+      for (int mt = m_first; mt < m_tiles; mt += ctas_per_n) {
+        for (int kb = 0; kb < num_kb; ++kb, ++it) {
+          const int s = it % kStages;
+          mbar_wait(&empty_bar[s], ((it / kStages) & 1) ^ 1);
+          mbar_expect_tx(&full_bar[s], 2 * Cfg::kTileBytes + Cfg::kBBytes);
+          tma_load_2d(smem_g + s * Cfg::kTileBytes, &tmap_g, &full_bar[s], kb * kBlockK, mt * kBlockM);
+          tma_load_2d(smem_y + s * Cfg::kTileBytes, &tmap_y, &full_bar[s], kb * kBlockK, mt * kBlockM);
+#pragma unroll
+          for (int b = 0; b < kBoxes; ++b)
+            tma_load_2d(smem_b + s * Cfg::kBBytes + b * 8192, &tmap_w, &full_bar[s], n0 + b * 64, kb * kBlockK);
+        }
+      }
+    }
+    return;
+  }
+
+  // ===== consumers: the coefficients of all K channels once per CTA (block 0 also writes dgamma / dbeta, as bn_bwd_apply)
+  const float inv_m = 1.f / (float)(int64_t)M;
+  for (int c = threadIdx.x; c < K; c += kConsumerThreads) {
+    const float sdz = gsum[c], sdzx = gsum[K + c];
+    const BnBwdCoef q = bn_bwd_coef(ld_w(bnw, wdt, c), saved[c], saved[K + c], sdz, sdzx, inv_m, (c & 7) == 7);
+    coef[c] = q.a; coef[K + c] = q.b; coef[2 * K + c] = q.d;
+    if (blockIdx.x == 0) { st_w(dw, wdt, c, sdzx); st_w(db, wdt, c, sdz); }
+  }
+  named_barrier(3, kConsumerThreads);
+
+  const int wg = warp >> 2, t = threadIdx.x & 127, w = warp & 3;
+  uint8_t* stg = smem_c + wg * (Cfg::kCBytes / 2);
+  float acc[BLOCK_N / 2] = {};
+  const int r0 = 16 * w + (lane >> 2);
+  // transform: thread t owns 16-byte granule j = t % 8 (channels 8j..8j+7 of the k-block) of rows t / 8 + 16 i of its warpgroup
+  const int j = t & 7, rbase = wg * 64 + (t >> 3);
+  const int mgroups = K / 8;
+
+  uint32_t it = 0;
+  for (int mt = m_first; mt < m_tiles; mt += ctas_per_n) {
+    for (int kb = 0; kb < num_kb; ++kb, ++it) {
+      const int s = it % kStages;
+      uint32_t bits[4] = {0u, 0u, 0u, 0u};
+      if constexpr (RELU) {
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+          const int row = mt * kBlockM + rbase + 16 * i;
+          if (row < M) bits[i] = mask[(size_t)row * mgroups + kb * 8 + j];
+        }
+      }
+      float ca[8], cb[8], cd[8];
+#pragma unroll
+      for (int e = 0; e < 8; ++e) {
+        const int c = kb * kBlockK + j * 8 + e;
+        ca[e] = coef[c]; cb[e] = coef[K + c]; cd[e] = coef[2 * K + c];
+      }
+      mbar_wait(&full_bar[s], (it / kStages) & 1);
+      uint8_t* gt = smem_g + s * Cfg::kTileBytes;
+      const uint8_t* yt = smem_y + s * Cfg::kTileBytes;
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        const int r = rbase + 16 * i;
+        const int off = r * 128 + ((j ^ (r & 7)) << 4);
+        uint4 gv = *reinterpret_cast<const uint4*>(gt + off);
+        const uint4 yv = *reinterpret_cast<const uint4*>(yt + off);
+        uint32_t* gw = reinterpret_cast<uint32_t*>(&gv);
+        const uint32_t* yw = reinterpret_cast<const uint32_t*>(&yv);
+#pragma unroll
+        for (int h = 0; h < 4; ++h) {
+          const float2 g2 = Wire<T>::unpack2(gw[h]), y2 = Wire<T>::unpack2(yw[h]);
+          float dz0 = g2.x, dz1 = g2.y;
+          if constexpr (RELU) {
+            dz0 = (bits[i] >> (2 * h)) & 1u ? dz0 : 0.f;
+            dz1 = (bits[i] >> (2 * h + 1)) & 1u ? dz1 : 0.f;
+          }
+          gw[h] = Wire<T>::pack2(bn_bwd_dx(ca[2 * h], cb[2 * h], cd[2 * h], dz0, y2.x),
+                                 bn_bwd_dx(ca[2 * h + 1], cb[2 * h + 1], cd[2 * h + 1], dz1, y2.y));
+        }
+        *reinterpret_cast<uint4*>(gt + off) = gv;
+      }
+      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // dx tile -> visible to wgmma and the TMA store
+      named_barrier(1 + wg, 128);
+      if (store_dx && t == 0) {
+        asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
+                     ::"l"(&tmap_dx), "r"(smem_u32(gt + wg * 64 * 128)), "r"(kb * kBlockK), "r"(mt * kBlockM + wg * 64) : "memory");
+        asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+      }
+      const uint64_t adesc = gmma_desc(gt + wg * 64 * 128);
+      const uint64_t bdesc = gmma_desc_mn(smem_b + s * Cfg::kBBytes);
+      fence_regs(acc);
+      asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
+#pragma unroll
+      for (int k = 0; k < kBlockK / 16; ++k) {
+        // one instruction covers the whole BLOCK_N; 16 k-rows of B are 2048 bytes further (+128 in the >>4 address field)
+        if constexpr (BLOCK_N == 128) wgmma_t128<T>(acc, adesc + 2 * k, bdesc + 128 * k, (kb | k) != 0);
+        else wgmma_t64<T>(acc, adesc + 2 * k, bdesc + 128 * k, (kb | k) != 0);
+      }
+      asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
+      asm volatile("wgmma.wait_group.sync.aligned 1;" ::: "memory");   // the previous stage's MMAs are done
+      fence_regs(acc);
+      if (kb > 0) {
+        if (store_dx && t == 0) asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory");   // its dx store has read it
+        if (lane == 0) mbar_arrive(&empty_bar[(it - 1) % kStages]);
+      }
+    }
+    asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
+    fence_regs(acc);
+    if (t == 0) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");   // last dx store and previous staging store
+    if (lane == 0) mbar_arrive(&empty_bar[(it - 1) % kStages]);
+
+    // ---- epilogue: the staged TMA store of gemm_bnstats_kernel, without the statistics
+    named_barrier(1 + wg, 128);
+#pragma unroll
+    for (int jj = 0; jj < BLOCK_N / 8; ++jj) {
+      uint8_t* box = stg + (jj >> 3) * 8192 + (lane & 3) * 4;
+      const int g = jj & 7;
+      *reinterpret_cast<uint32_t*>(box + r0 * 128 + ((g ^ (r0 & 7)) << 4)) = Wire<T>::pack2(acc[4 * jj], acc[4 * jj + 1]);
+      *reinterpret_cast<uint32_t*>(box + (r0 + 8) * 128 + ((g ^ (r0 & 7)) << 4)) = Wire<T>::pack2(acc[4 * jj + 2], acc[4 * jj + 3]);
+    }
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+    named_barrier(1 + wg, 128);
+    if (t == 0) {
+#pragma unroll
+      for (int b = 0; b < kBoxes; ++b)
+        asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
+                     ::"l"(&tmap_c), "r"(smem_u32(stg + b * 8192)), "r"(n0 + b * 64), "r"(mt * kBlockM + wg * 64) : "memory");
+      asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+    }
+  }
+  if (t == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
+}
+
 // ------------------------------------------------------------------ host
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*, const cuuint32_t*,
                                   const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
@@ -288,6 +512,8 @@ static CUtensorMap make_map(CUtensorMapDataType dtype, const void* ptr, int64_t 
   TORCH_CHECK(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled failed: ", (int)r);
   return m;
 }
+
+template <typename T> struct TypeTag { using type = T; };
 
 template <typename T, int BLOCK_N>
 static void launch_gemm(const at::Tensor& a, const at::Tensor& b, at::Tensor& c, at::Tensor& gsum, int M, int N, int K, const SyncBN* sync) {
@@ -342,6 +568,57 @@ at::Tensor conv1x1_bnstats(const at::Tensor& x, const at::Tensor& weight, at::Te
   if (x.scalar_type() == at::kHalf) launch_gemm_for<__half>(x, w2, y, gsum, M, N, K, sync);
   else launch_gemm_for<__nv_bfloat16>(x, w2, y, gsum, M, N, K, sync);
   return y;
+}
+
+template <typename T, int BLOCK_N, bool RELU>
+static void launch_dgrad(const at::Tensor& g, const at::Tensor& y, const uint8_t* mask, const at::Tensor& saved, const float* sums,
+                         const at::Tensor& bnw, int wdt, at::Tensor& dw, at::Tensor& db, const at::Tensor& w2, at::Tensor& dx, at::Tensor& din,
+                         int M, int N, int K) {
+  constexpr int smem = DgradCfg<BLOCK_N>::kSmem;
+  auto kernel = gemm_bnbwd_dgrad_kernel<T, BLOCK_N, RELU>;
+  static bool configured[64] = {};
+  const int dev = g.get_device();
+  if (!configured[dev & 63]) {
+    C10_CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    configured[dev & 63] = true;
+  }
+  constexpr CUtensorMapDataType dt = std::is_same<T, __half>::value ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
+  const CUtensorMap mg = make_map(dt, g.data_ptr(), M, K, kBlockM, CU_TENSOR_MAP_L2_PROMOTION_L2_256B);
+  const CUtensorMap my = make_map(dt, y.data_ptr(), M, K, kBlockM, CU_TENSOR_MAP_L2_PROMOTION_L2_256B);
+  const CUtensorMap mw = make_map(dt, w2.data_ptr(), K, N, 64, CU_TENSOR_MAP_L2_PROMOTION_L2_256B);    // [K, N]: 64 k-rows x 64 n
+  const CUtensorMap mdx = make_map(dt, dx.data_ptr(), M, K, 64, CU_TENSOR_MAP_L2_PROMOTION_NONE);
+  const CUtensorMap mc = make_map(dt, din.data_ptr(), M, N, 64, CU_TENSOR_MAP_L2_PROMOTION_NONE);
+  const int m_tiles = (M + kBlockM - 1) / kBlockM, n_tiles = N / BLOCK_N;
+  const int sms = at::cuda::getCurrentDeviceProperties()->multiProcessorCount;
+  const int ctas_per_n = std::max(1, std::min(m_tiles, sms / n_tiles));
+  kernel<<<ctas_per_n * n_tiles, kGemmThreads, smem, at::cuda::getCurrentCUDAStream()>>>(
+      mg, my, mw, mdx, mc, mask, saved.data_ptr<float>(), sums, bnw.data_ptr(), wdt, dw.data_ptr(), db.data_ptr(), M, K, m_tiles, n_tiles,
+      ctas_per_n);
+  C10_CUDA_KERNEL_LAUNCH_CHECK();
+}
+
+void conv1x1_dgrad_bn(const at::Tensor& g, const at::Tensor& y, const uint8_t* mask, const at::Tensor& saved, const float* sums,
+                      const at::Tensor& bnw, int wdt, at::Tensor& dw, at::Tensor& db, const at::Tensor& conv_w, at::Tensor& dx, at::Tensor& din) {
+  const int64_t M64 = y.size(0) * y.size(2) * y.size(3);
+  const int K = (int)y.size(1), N = (int)conv_w.size(1);
+  TORCH_CHECK(conv_w.dim() == 4 && conv_w.size(0) == K && conv_w.size(2) == 1 && conv_w.size(3) == 1 && conv_w.scalar_type() == y.scalar_type(),
+              "conv1x1_bn_backward: the conv weight must be [C_out, C_in, 1, 1] with the activations' dtype");
+  TORCH_CHECK(K % kBlockK == 0 && K <= kCoefMaxK && N % 64 == 0 && M64 < (int64_t)1 << 31, "conv1x1_bn_backward: unsupported shape");
+  at::Tensor w2 = conv_w.reshape({K, N});
+  TORCH_CHECK(w2.is_contiguous(), "conv1x1_bn_backward: the conv weight must be dense [C_out, C_in]");
+  const int M = (int)M64;
+  auto run = [&](auto tag) {
+    using T = typename decltype(tag)::type;
+    if (N % 128 == 0) {
+      if (mask) launch_dgrad<T, 128, true>(g, y, mask, saved, sums, bnw, wdt, dw, db, w2, dx, din, M, N, K);
+      else launch_dgrad<T, 128, false>(g, y, mask, saved, sums, bnw, wdt, dw, db, w2, dx, din, M, N, K);
+    } else {
+      if (mask) launch_dgrad<T, 64, true>(g, y, mask, saved, sums, bnw, wdt, dw, db, w2, dx, din, M, N, K);
+      else launch_dgrad<T, 64, false>(g, y, mask, saved, sums, bnw, wdt, dw, db, w2, dx, din, M, N, K);
+    }
+  };
+  if (y.scalar_type() == at::kHalf) run(TypeTag<__half>{});
+  else run(TypeTag<__nv_bfloat16>{});
 }
 
 }  // namespace ptd

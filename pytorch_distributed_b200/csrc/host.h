@@ -74,6 +74,11 @@ std::vector<at::Tensor> bn_act_backward(const at::Tensor& dy, const at::Tensor& 
 std::vector<at::Tensor> bn_act_backward2(const at::Tensor& dy_a, const at::Tensor& dy_b, const at::Tensor& x,
                                          const c10::optional<at::Tensor>& mask, const at::Tensor& weight, const at::Tensor& saved, bool relu,
                                          at::Tensor work, const SyncBN* sync);
+// The backward of a 1x1 conv -> BatchNorm pair of one rank: the reduction pass, then gemm_bnstats.cu's data-gradient GEMM that
+// applies the BatchNorm backward to its A operand.  returns {d conv input, dx, g (with dy_b), dweight, dbias}
+std::vector<at::Tensor> conv1x1_bn_backward(const at::Tensor& dy_a, const c10::optional<at::Tensor>& dy_b, const at::Tensor& y,
+                                            const c10::optional<at::Tensor>& mask, const at::Tensor& weight, const at::Tensor& saved,
+                                            const at::Tensor& conv_weight, bool relu, at::Tensor work);
 
 std::vector<at::Tensor> stem_forward(const at::Tensor& x, const at::Tensor& weight, const at::Tensor& bias, at::Tensor running_mean,
                                      at::Tensor running_var, c10::optional<at::Tensor> num_batches_tracked, bool training, double momentum,
@@ -101,6 +106,11 @@ float* finish_sums(const float* part, int nblocks, int C, int64_t rows, float* w
 
 // ---- gemm_bnstats.cu (wgmma / TMA)
 at::Tensor conv1x1_bnstats(const at::Tensor& x, const at::Tensor& weight, at::Tensor gsum, const SyncBN* sync);
+// dIn = dx x W with dx = bn_bwd_dx(A, B, D, g (x mask bits), y) formed in shared memory and also written to `dx`; A / B / D
+// from saved, sums and bnw (dtype wdt), which block 0 also writes as dw / db (as bn_bwd_apply does).  mask: nullptr, or the
+// forward's ReLU bits.  conv_w: [K, N, 1, 1], dx: [M, K], din: [M, N], all channels_last.
+void conv1x1_dgrad_bn(const at::Tensor& g, const at::Tensor& y, const uint8_t* mask, const at::Tensor& saved, const float* sums,
+                      const at::Tensor& bnw, int wdt, at::Tensor& dw, at::Tensor& db, const at::Tensor& conv_w, at::Tensor& dx, at::Tensor& din);
 
 // ---- stem_conv.cu
 at::Tensor stem_im2col(const at::Tensor& x);
