@@ -105,6 +105,15 @@ def build_parser(entry: str = "distributed") -> argparse.ArgumentParser:
                         "validate it after each epoch and save it as state_dict_ema")
     x.add_argument("--model-ema-decay", default=None, type=float, metavar="D",
                    help="decay of --model-ema: e = D e + (1 - D) p after every optimizer step, 0 <= D < 1 (default: 0.9999)")
+    x.add_argument("--label-smoothing", default=0.0, type=_unit_float, metavar="EPS",
+                   help="cross-entropy against (1 - EPS) target + EPS / classes, 0 <= EPS <= 1 (torch's label_smoothing; "
+                        "default: 0.0)")
+    x.add_argument("--mixup-alpha", default=0.0, type=_alpha, metavar="A",
+                   help="MixUp with lambda ~ Beta(A, A) on every training batch, as torchvision's transforms.v2.MixUp; one pass "
+                        "of a fused kernel on the GPU (default: 0.0 = off)")
+    x.add_argument("--cutmix-alpha", default=0.0, type=_alpha, metavar="A",
+                   help="CutMix with lambda ~ Beta(A, A), as torchvision's transforms.v2.CutMix; with --mixup-alpha too, each "
+                        "batch takes one of the two at random (default: 0.0 = off)")
     x.add_argument("--cuda-graph", action="store_true", help="capture the train step in a CUDA graph")
     x.add_argument("--sync-bn", action="store_true",
                    help="synchronise BatchNorm statistics across the data-parallel ranks (torch.nn.SyncBatchNorm semantics; "
@@ -144,6 +153,20 @@ def _positive_float(s: str) -> float:
     v = float(s)
     if not (v > 0 and math.isfinite(v)):
         raise argparse.ArgumentTypeError("must be a positive finite number, got %r" % (s,))
+    return v
+
+
+def _unit_float(s: str) -> float:
+    v = float(s)
+    if not 0.0 <= v <= 1.0:
+        raise argparse.ArgumentTypeError("must lie in [0, 1], got %r" % (s,))
+    return v
+
+
+def _alpha(s: str) -> float:
+    v = float(s)
+    if not (v >= 0 and math.isfinite(v)):
+        raise argparse.ArgumentTypeError("must be a finite number >= 0, got %r" % (s,))
     return v
 
 

@@ -154,6 +154,9 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("resample_normalize", &resample_normalize, py::arg("arena"), py::arg("n"), py::arg("out_h"), py::arg("out_w"), py::arg("max_rows"),
         py::arg("a"), py::arg("b"), py::arg("out_dtype"), py::arg("channels_last"));
   m.def("p2p_copy_multi", &p2p_copy_multi);
+  m.def("mix_batch", &mix_batch, py::arg("x"), py::arg("out"), py::arg("y"), py::arg("yb"), py::arg("dom"), py::arg("prm"));
+  m.def("soft_ce_fwd", &soft_ce_fwd, py::arg("z"), py::arg("ya"), py::arg("yb"), py::arg("prm"), py::arg("eps"));
+  m.def("soft_ce_bwd", &soft_ce_bwd, py::arg("z"), py::arg("ya"), py::arg("yb"), py::arg("prm"), py::arg("lse"), py::arg("g"), py::arg("eps"));
 
   // horovod-style fusion queue (background thread + tensor fusion scheduling), see hvd_core.cpp
   py::class_<FusionQueue, std::shared_ptr<FusionQueue>>(m, "FusionQueue")

@@ -124,4 +124,13 @@ void p2p_copy_multi(std::vector<at::Tensor> src, std::vector<at::Tensor> dst, in
 at::Tensor resample_normalize(const at::Tensor& arena, int64_t n, int64_t out_h, int64_t out_w, int64_t max_rows, const at::Tensor& a,
                               const at::Tensor& b, int64_t out_dtype, bool channels_last);
 
+// ---- mix.cu (prm: the float[8] per-step parameters, see mix.cu)
+// out = MixUp / CutMix of x with roll(x, 1, 0); yb = roll(y, 1); dom = the argmax label of the mixed target
+void mix_batch(const at::Tensor& x, at::Tensor out, const at::Tensor& y, at::Tensor yb, at::Tensor dom, const at::Tensor& prm);
+// cross-entropy against (1-eps)(la onehot(ya) + lb onehot(yb)) + eps/C: returns {mean loss, per-row loss, per-row lse}
+std::vector<at::Tensor> soft_ce_fwd(const at::Tensor& z, const at::Tensor& ya, const at::Tensor& yb, const at::Tensor& prm, double eps);
+// dz = g[0] / B (softmax(z) - q), in the logits' dtype
+at::Tensor soft_ce_bwd(const at::Tensor& z, const at::Tensor& ya, const at::Tensor& yb, const at::Tensor& prm, const at::Tensor& lse,
+                       const at::Tensor& g, double eps);
+
 }  // namespace ptd

@@ -201,11 +201,16 @@ class TrainStep:
     no-sync context; call N runs the body above with loss / N.  The metrics keep the undivided loss.  Under a graph each
     of the two kinds of pass is captured the first time it comes after the warm-up and one eager optimizer step (two
     graphs, one memory pool).
+
+    MixUp / CutMix / label smoothing (``st.batch_mix``, an :class:`~.ops.mix.BatchMix`): every pass draws its mixing
+    parameters on the host first (eager, and before each replay), mixes the batch, takes the loss from
+    ``batch_mix.loss`` and gives the metric kernel the dominant labels.  The ``criterion`` passed in is then unused.
     """
 
     def __init__(self, st, model, criterion, optimizer, metrics, use_graph: bool = False, warmup: int = 3, ema=None):
         self.st, self.model, self.criterion, self.optimizer, self.metrics = st, model, criterion, optimizer, metrics
         self.ema = ema if ema is not None else getattr(st, "model_ema", None)   # --model-ema: once per optimizer step
+        self.batch_mix = getattr(st, "batch_mix", None)
         self.use_graph = bool(use_graph) and torch.cuda.is_available()
         self.warmup = warmup
         self.calls = 0
@@ -221,8 +226,15 @@ class TrainStep:
         nvtx = _NVTX and images.is_cuda          # PTD_NVTX=1: forward / backward(+bucket all-reduce) / optimizer ranges for nsys / ncu
         if nvtx:
             torch.cuda.nvtx.range_push("ptd.forward")
+        bm = self.batch_mix
+        if bm is not None:
+            images, mixed = bm.apply(images, target)
         output = self.st.forward(self.model, images)
-        loss = self.criterion(output.float() if output.dtype != torch.float32 else output, target)
+        if bm is not None:
+            loss = bm.loss(output, mixed)
+            target = bm.metric_target(mixed)
+        else:
+            loss = self.criterion(output.float() if output.dtype != torch.float32 else output, target)
         if dev is None:
             self.metrics.push(output, target, loss, images.size(0))
         else:
@@ -289,6 +301,8 @@ class TrainStep:
     def __call__(self, images, target):
         self.calls += 1
         last = self.k == self.accum - 1
+        if self.batch_mix is not None:
+            self.batch_mix.draw(images.shape[-2:])
         # with accumulation, capture after one eager optimizer step (it creates the optimizer's device state, a host copy
         # no capture may hold) and the earlier-pass graph first: a last pass that adds into p.grad through autograd
         # (horovod's backward_passes_per_step) must be captured reading the gradients that graph writes
@@ -408,9 +422,11 @@ class Strategy:
         return model
 
     def build(self, model, args, device, local_rank):
-        """Precision, wrapper and optimizer (``build_model``), then the ``--model-ema`` average of the finished model."""
+        """Precision, wrapper and optimizer (``build_model``), then the ``--model-ema`` average of the finished model and the
+        ``--label-smoothing`` / ``--mixup-alpha`` / ``--cutmix-alpha`` target policy."""
         model, optimizer = self.build_model(model, args, device, local_rank)
         self.model_ema = make_model_ema(model, optimizer, args)
+        self.batch_mix = make_batch_mix(args, device, self.rank() if self.distributed else 0)
         return model, optimizer
 
     def build_model(self, model, args, device, local_rank):
@@ -604,6 +620,8 @@ def main_worker(local_rank: int, nprocs: int, args, strategy: Optional[Strategy]
         args.batch_size = max(1, int(args.batch_size / world))
     model, optimizer = st.build(model, args, device, local_rank)
     criterion = nn.CrossEntropyLoss().to(device)
+    bm = getattr(st, "batch_mix", None)
+    val_criterion = bm.criterion if bm is not None else criterion     # validation: label smoothing, never mixing
     torch.backends.cudnn.benchmark = True
 
     train_loader, val_loader, train_sampler, val_sampler = build_loaders(args, args.batch_size, distributed=st.distributed,
@@ -625,9 +643,9 @@ def main_worker(local_rank: int, nprocs: int, args, strategy: Optional[Strategy]
                 print("=> no state_dict_ema in checkpoint '{}': the EMA starts from the resumed weights".format(args.resume))
 
     if args.evaluate:
-        validate(val_loader, model, criterion, st, device, args)
+        validate(val_loader, model, val_criterion, st, device, args)
         if ema is not None:
-            validate_ema(ema, val_loader, criterion, st, device, args)
+            validate_ema(ema, val_loader, val_criterion, st, device, args)
         _shutdown(st)
         return
 
@@ -635,11 +653,13 @@ def main_worker(local_rank: int, nprocs: int, args, strategy: Optional[Strategy]
         t_epoch = time.time()
         train_sampler.set_epoch(epoch)
         val_sampler.set_epoch(epoch)
+        if bm is not None:
+            bm.set_epoch(epoch)
         adjust_learning_rate(optimizer, epoch, args)
         train(train_loader, model, criterion, optimizer, epoch, st, device, args)
-        acc1 = validate(val_loader, model, criterion, st, device, args)
+        acc1 = validate(val_loader, model, val_criterion, st, device, args)
         if ema is not None:
-            validate_ema(ema, val_loader, criterion, st, device, args)
+            validate_ema(ema, val_loader, val_criterion, st, device, args)
         is_best = acc1 > best_acc1          # model_best follows the live model's Acc@1
         best_acc1 = max(acc1, best_acc1)
         if st.epoch_csv and st.is_saver(args):
@@ -666,6 +686,15 @@ def make_model_ema(model, optimizer, args):
         return None
     from .utils.ema import ModelEma
     return ModelEma(model, decay=args.model_ema_decay, optimizer=optimizer)
+
+
+def make_batch_mix(args, device, rank: int):
+    """``--label-smoothing`` / ``--mixup-alpha`` / ``--cutmix-alpha``: the BatchMix of this rank (None when all three are 0)."""
+    eps, mix, cut = (float(getattr(args, k, 0.0) or 0.0) for k in ("label_smoothing", "mixup_alpha", "cutmix_alpha"))
+    if not (eps or mix or cut):
+        return None
+    from .ops.mix import BatchMix
+    return BatchMix(mix, cut, eps, num_classes=args.num_classes, seed=args.seed, rank=rank, device=device)
 
 
 def validate_ema(ema, val_loader, criterion, st, device, args):
