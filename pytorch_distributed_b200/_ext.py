@@ -22,7 +22,7 @@ _NAME = "_C"
 _SO = os.path.join(_HERE, _NAME + ".so")
 _STAMP = os.path.join(_HERE, _NAME + ".hash")
 _SOURCES = ["bindings.cpp", "symm.cpp", "hvd_core.cpp", "collectives.cu", "optim.cu", "bn_act.cu", "data_ops.cu", "gemm_bnstats.cu", "stem_conv.cu",
-            "resample.cu", "sync_bn.cu", "mix.cu"]
+            "resample.cu", "sync_bn.cu", "mix.cu", "augment.cu"]
 _lock = threading.Lock()
 _mod = None
 _err = None

@@ -114,6 +114,12 @@ def build_parser(entry: str = "distributed") -> argparse.ArgumentParser:
     x.add_argument("--cutmix-alpha", default=0.0, type=_alpha, metavar="A",
                    help="CutMix with lambda ~ Beta(A, A), as torchvision's transforms.v2.CutMix; with --mixup-alpha too, each "
                         "batch takes one of the two at random (default: 0.0 = off)")
+    x.add_argument("--auto-augment", default=None, choices=["ta_wide"],
+                   help="per-sample TrivialAugment Wide on the training crops, as torchvision's transforms.v2.TrivialAugmentWide "
+                        "(bilinear); fused into the normalising kernel on the GPU (default: none)")
+    x.add_argument("--random-erase", default=0.0, type=_unit_float, metavar="P",
+                   help="erase a random box of each training image with probability P, as torchvision's RandomErasing(P) after "
+                        "the normalisation (default: 0.0)")
     x.add_argument("--cuda-graph", action="store_true", help="capture the train step in a CUDA graph")
     x.add_argument("--sync-bn", action="store_true",
                    help="synchronise BatchNorm statistics across the data-parallel ranks (torch.nn.SyncBatchNorm semantics; "

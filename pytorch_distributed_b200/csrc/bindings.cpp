@@ -153,6 +153,11 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("normalize_nhwc", &normalize_nhwc);
   m.def("resample_normalize", &resample_normalize, py::arg("arena"), py::arg("n"), py::arg("out_h"), py::arg("out_w"), py::arg("max_rows"),
         py::arg("a"), py::arg("b"), py::arg("out_dtype"), py::arg("channels_last"));
+  m.attr("U8_OUT") = kU8Out;
+  m.def("augment_normalize", &augment_normalize, py::arg("src"), py::arg("prm"), py::arg("a"), py::arg("b"), py::arg("out_dtype"),
+        py::arg("channels_last"));
+  m.attr("AUG_PRM") = kAugPrm;
+  m.attr("AUG_MAX_PIXELS") = kAugMaxPixels;
   m.def("p2p_copy_multi", &p2p_copy_multi);
   m.def("mix_batch", &mix_batch, py::arg("x"), py::arg("out"), py::arg("y"), py::arg("yb"), py::arg("dom"), py::arg("prm"));
   m.def("soft_ce_fwd", &soft_ce_fwd, py::arg("z"), py::arg("ya"), py::arg("yb"), py::arg("prm"), py::arg("eps"));

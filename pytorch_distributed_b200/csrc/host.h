@@ -120,7 +120,8 @@ at::Tensor normalize_nhwc(const at::Tensor& src, const at::Tensor& mean, const a
 
 void p2p_copy_multi(std::vector<at::Tensor> src, std::vector<at::Tensor> dst, int64_t run_device);
 
-// ---- resample.cu
+// ---- resample.cu (out_dtype kU8Out: the rounded uint8 pixels, NCHW, without the normalisation)
+constexpr int64_t kU8Out = 3;
 at::Tensor resample_normalize(const at::Tensor& arena, int64_t n, int64_t out_h, int64_t out_w, int64_t max_rows, const at::Tensor& a,
                               const at::Tensor& b, int64_t out_dtype, bool channels_last);
 
@@ -132,5 +133,12 @@ std::vector<at::Tensor> soft_ce_fwd(const at::Tensor& z, const at::Tensor& ya, c
 // dz = g[0] / B (softmax(z) - q), in the logits' dtype
 at::Tensor soft_ce_bwd(const at::Tensor& z, const at::Tensor& ya, const at::Tensor& yb, const at::Tensor& prm, const at::Tensor& lse,
                        const at::Tensor& g, double eps);
+
+// ---- augment.cu (prm: float32 [n, kAugPrm], one row of encoded op parameters per sample, see augment.cu)
+// TrivialAugmentWide + normalise + RandomErasing of a uint8 NCHW batch; returns what normalize_nhwc returns for it unaugmented
+constexpr int64_t kAugPrm = 16;
+constexpr int64_t kAugMaxPixels = 65793;      // 255 H W < 2^24: Contrast's float32 grayscale sum is exact in any order
+at::Tensor augment_normalize(const at::Tensor& src, const at::Tensor& prm, const at::Tensor& a, const at::Tensor& b, int64_t out_dtype,
+                             bool channels_last);
 
 }  // namespace ptd

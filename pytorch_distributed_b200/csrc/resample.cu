@@ -36,6 +36,9 @@ constexpr int kThreads = 256;
 constexpr int kBandRows = 16;
 constexpr int kSmemTarget = 64 << 10;      // 3 CTAs per SM; at out_w = 224 it holds 24 resampled rows
 
+template <typename Out> __device__ __forceinline__ Out out_px(float v) { return from_f32<Out>(v); }
+template <> __device__ __forceinline__ uint8_t out_px<uint8_t>(float v) { return (uint8_t)v; }
+
 template <typename Out, bool NHWC_OUT>
 __global__ void __launch_bounds__(kThreads) resample_normalize_kernel(const uint8_t* __restrict__ arena, Out* __restrict__ dst,
                                                                       const float* __restrict__ na, const float* __restrict__ nb,
@@ -101,17 +104,17 @@ __global__ void __launch_bounds__(kThreads) resample_normalize_kernel(const uint
 #pragma unroll
       for (int c = 0; c < 3; ++c) {
         const float px = (float)__float2uint_rz(fminf(255.f, fmaxf(0.f, __fadd_rn(acc[c], 0.5f))));
-        v[c] = __fmaf_rn(px, sa[c], sb[c]);
+        v[c] = std::is_same<Out, uint8_t>::value ? px : __fmaf_rn(px, sa[c], sb[c]);   // uint8: the pixel itself
       }
       const size_t pix = (size_t)o * out_w + x;
       if constexpr (NHWC_OUT) {
         Out* q = dst + ((size_t)s * plane + pix) * 3;
 #pragma unroll
-        for (int c = 0; c < 3; ++c) q[c] = from_f32<Out>(v[c]);
+        for (int c = 0; c < 3; ++c) q[c] = out_px<Out>(v[c]);
       } else {
         Out* q = dst + (size_t)s * 3 * plane + pix;
 #pragma unroll
-        for (int c = 0; c < 3; ++c) q[c * plane] = from_f32<Out>(v[c]);
+        for (int c = 0; c < 3; ++c) q[c * plane] = out_px<Out>(v[c]);
       }
     }
     __syncthreads();
@@ -135,7 +138,8 @@ void launch(const at::Tensor& arena, at::Tensor& dst, const at::Tensor& a, const
 
 // arena: a staged batch copied to the device (descriptors of samples 0..n-1 first).  max_rows: an upper bound of the
 // y tap counts (ShardLoader.stage_max_rows()).  Returns the tensor normalize_nhwc returns for the host-resampled batch: [n, 3, out_h, out_w] of
-// (pixel * a[c] + b[c]) in out_dtype, channels_last or contiguous.
+// (pixel * a[c] + b[c]) in out_dtype, channels_last or contiguous.  out_dtype kU8Out returns the uint8 batch itself (contiguous
+// NCHW, no normalisation): the input of augment_normalize, the same bytes as the host-resampled batch.
 at::Tensor resample_normalize(const at::Tensor& arena, int64_t n, int64_t out_h, int64_t out_w, int64_t max_rows, const at::Tensor& a,
                               const at::Tensor& b, int64_t out_dtype, bool channels_last) {
   TORCH_CHECK(arena.is_cuda() && arena.scalar_type() == at::kByte && arena.dim() == 1 && arena.is_contiguous(),
@@ -150,10 +154,12 @@ at::Tensor resample_normalize(const at::Tensor& arena, int64_t n, int64_t out_h,
   C10_CUDA_CHECK(cudaDeviceGetAttribute(&smem_max, cudaDevAttrMaxSharedMemoryPerBlockOptin, arena.get_device()));
   TORCH_CHECK((int64_t)cap_rows * row_bytes <= smem_max, "resample_normalize: ", cap_rows, " source rows of width ", out_w,
               " do not fit in shared memory");
-  const at::ScalarType ot = out_dtype == kBF16 ? at::kBFloat16 : out_dtype == kF16 ? at::kHalf : at::kFloat;
+  const at::ScalarType ot = out_dtype == kU8Out ? at::kByte : out_dtype == kBF16 ? at::kBFloat16 : out_dtype == kF16 ? at::kHalf : at::kFloat;
+  TORCH_CHECK(!(ot == at::kByte && channels_last), "resample_normalize: the uint8 output is NCHW");
   at::Tensor dst = at::empty({n, 3, out_h, out_w}, arena.options().dtype(ot).memory_format(channels_last ? at::MemoryFormat::ChannelsLast
                                                                                                         : at::MemoryFormat::Contiguous));
   switch (ot) {
+    case at::kByte: launch<uint8_t>(arena, dst, a, b, (int)n, (int)out_h, (int)out_w, cap_rows, false); break;
     case at::kBFloat16: launch<__nv_bfloat16>(arena, dst, a, b, (int)n, (int)out_h, (int)out_w, cap_rows, channels_last); break;
     case at::kHalf: launch<__half>(arena, dst, a, b, (int)n, (int)out_h, (int)out_w, cap_rows, channels_last); break;
     default: launch<float>(arena, dst, a, b, (int)n, (int)out_h, (int)out_w, cap_rows, channels_last); break;

@@ -423,10 +423,12 @@ class Strategy:
 
     def build(self, model, args, device, local_rank):
         """Precision, wrapper and optimizer (``build_model``), then the ``--model-ema`` average of the finished model and the
-        ``--label-smoothing`` / ``--mixup-alpha`` / ``--cutmix-alpha`` target policy."""
+        ``--label-smoothing`` / ``--mixup-alpha`` / ``--cutmix-alpha`` target policy and the ``--auto-augment`` /
+        ``--random-erase`` input policy."""
         model, optimizer = self.build_model(model, args, device, local_rank)
         self.model_ema = make_model_ema(model, optimizer, args)
         self.batch_mix = make_batch_mix(args, device, self.rank() if self.distributed else 0)
+        self.batch_augment = make_batch_augment(args, device, self.rank() if self.distributed else 0)
         return model, optimizer
 
     def build_model(self, model, args, device, local_rank):
@@ -447,10 +449,12 @@ class Strategy:
     def unwrapped(self, model):
         return model.module if hasattr(model, "module") else model
 
-    def prefetcher(self, loader, device, args, limit=None):
+    def prefetcher(self, loader, device, args, limit=None, augment=None):
+        """``augment``: the training loader's :class:`~.ops.augment.BatchAugment`, applied when the loader ships uint8 pixels
+        (ImageFolder workers that normalise have applied torchvision's transforms already)."""
         raw = self.raw_uint8_loader or getattr(loader, "raw_uint8", False)     # native shard loader ships uint8 pixels
         return DataPrefetcher(loader, device, dtype=self.input_dtype, channels_last=bool(args.channels_last),
-                              normalize="imagenet255" if raw else None, limit=limit)
+                              normalize="imagenet255" if raw else None, limit=limit, augment=augment if raw else None)
 
 
 class ApexStrategy(Strategy):
@@ -655,6 +659,8 @@ def main_worker(local_rank: int, nprocs: int, args, strategy: Optional[Strategy]
         val_sampler.set_epoch(epoch)
         if bm is not None:
             bm.set_epoch(epoch)
+        if getattr(st, "batch_augment", None) is not None:
+            st.batch_augment.set_epoch(epoch)
         adjust_learning_rate(optimizer, epoch, args)
         train(train_loader, model, criterion, optimizer, epoch, st, device, args)
         acc1 = validate(val_loader, model, val_criterion, st, device, args)
@@ -695,6 +701,15 @@ def make_batch_mix(args, device, rank: int):
         return None
     from .ops.mix import BatchMix
     return BatchMix(mix, cut, eps, num_classes=args.num_classes, seed=args.seed, rank=rank, device=device)
+
+
+def make_batch_augment(args, device, rank: int):
+    """``--auto-augment`` / ``--random-erase``: the BatchAugment of this rank (None when both are off)."""
+    policy, p = getattr(args, "auto_augment", None), float(getattr(args, "random_erase", 0.0) or 0.0)
+    if policy is None and not p:
+        return None
+    from .ops.augment import BatchAugment
+    return BatchAugment(policy, p, seed=args.seed, rank=rank)
 
 
 def validate_ema(ema, val_loader, criterion, st, device, args):
@@ -785,7 +800,7 @@ def train(train_loader, model, criterion, optimizer, epoch, st: Strategy, device
         # whole optimizer steps only: a group of micro-batches never crosses an epoch (or the checkpoint written after it)
         n = len(train_loader) if limit is None else min(len(train_loader), limit)
         limit = n // accum * accum
-    pf = st.prefetcher(train_loader, device, args, limit=limit)
+    pf = st.prefetcher(train_loader, device, args, limit=limit, augment=getattr(st, "batch_augment", None))
     progress = ProgressMeter(len(pf), [batch_time, data_time, losses, top1, top5], prefix="Epoch: [{}]".format(epoch))
     metrics = MetricPipeline(getattr(st, "comm", None), device, (losses, top1, top5), reduce=st.reduce_metrics)
     model.train()

@@ -43,6 +43,7 @@ class SyntheticLoader:
     def __init__(self, batch_size: int, steps: int, image_size: int = 224, num_classes: int = 1000, pool: int = 4,
                  seed: int = 0, raw_uint8: bool = False, pin: Optional[bool] = None, rank: int = 0):
         self.batch_size, self.steps = int(batch_size), int(steps)
+        self.raw_uint8 = bool(raw_uint8)
         self.sampler = _EpochSampler()
         g = torch.Generator().manual_seed(1234 + seed * 7919 + rank * 104729)
         pin = torch.cuda.is_available() if pin is None else pin
@@ -70,9 +71,18 @@ def _world():
     return (dist.get_rank(), dist.get_world_size()) if dist.is_available() and dist.is_initialized() else (0, 1)
 
 
+def augmenting(args) -> bool:
+    """``--auto-augment`` or ``--random-erase`` is on."""
+    return getattr(args, "auto_augment", None) is not None or float(getattr(args, "random_erase", 0.0) or 0.0) > 0
+
+
 def build_loaders(args, batch_size: int, distributed: bool = True, raw_uint8: bool = False):
-    """(train_loader, val_loader, train_sampler, val_sampler) for this rank.  ``batch_size`` is per loader."""
+    """(train_loader, val_loader, train_sampler, val_sampler) for this rank.  ``batch_size`` is per loader.
+
+    With ``--auto-augment`` / ``--random-erase``: shard and synthetic training batches are uint8 (the prefetcher augments
+    them on the device, ``ops/augment.py``), and ``ImageFolder`` workers run torchvision's transforms themselves."""
     rank, world = _world() if distributed else (0, 1)
+    aug = augmenting(args)
     if args.data and not args.synthetic:
         from . import shards
         if shards.find_shards(args.data, "train"):          # pre-decoded shards -> native C++ loader (always uint8 batches)
@@ -85,15 +95,14 @@ def build_loaders(args, batch_size: int, distributed: bool = True, raw_uint8: bo
         tsteps = args.steps_per_epoch or max(1, math.ceil(n_train / shards / batch_size))
         vsteps = args.val_steps or args.steps_per_epoch or max(1, math.ceil(n_val / shards / batch_size))
         seed = args.seed or 0
-        train = SyntheticLoader(batch_size, tsteps, args.image_size, args.num_classes, seed=seed, raw_uint8=raw_uint8, rank=rank)
+        train = SyntheticLoader(batch_size, tsteps, args.image_size, args.num_classes, seed=seed, raw_uint8=raw_uint8 or aug, rank=rank)
         val = SyntheticLoader(batch_size, vsteps, args.image_size, args.num_classes, seed=seed + 1, raw_uint8=raw_uint8, rank=rank)
         return train, val, train.sampler, val.sampler
     import torchvision.datasets as datasets
     import torchvision.transforms as transforms
     normalize = transforms.Normalize(mean=IMAGENET_MEAN, std=IMAGENET_STD)
     tail = [transforms.PILToTensor()] if raw_uint8 else [transforms.ToTensor(), normalize]
-    train_ds = datasets.ImageFolder(os.path.join(args.data, "train"), transforms.Compose(
-        [transforms.RandomResizedCrop(args.image_size), transforms.RandomHorizontalFlip()] + tail))
+    train_ds = datasets.ImageFolder(os.path.join(args.data, "train"), transforms.Compose(train_transforms(args, raw_uint8)))
     val_ds = datasets.ImageFolder(os.path.join(args.data, "val"), transforms.Compose(
         [transforms.Resize(int(args.image_size * 256 / 224)), transforms.CenterCrop(args.image_size)] + tail))
     if distributed and world > 1:
@@ -109,6 +118,23 @@ def build_loaders(args, batch_size: int, distributed: bool = True, raw_uint8: bo
     val = torch.utils.data.DataLoader(val_ds, batch_size=batch_size, shuffle=False, num_workers=args.workers, pin_memory=pin,
                                       sampler=vs, persistent_workers=args.workers > 0)
     return train, val, ts or _EpochSampler(), vs or _EpochSampler()
+
+
+def train_transforms(args, raw_uint8: bool = False):
+    """The ``ImageFolder`` training transforms: the crop and flip, then (``--auto-augment ta_wide``) TrivialAugmentWide on the
+    crop and (``--random-erase P``) RandomErasing after ``Normalize``, in the order of torchvision's classification recipe.
+    With ``raw_uint8`` the workers ship uint8 tensors and the prefetcher normalises and augments them."""
+    import torchvision.transforms as transforms
+    t = [transforms.RandomResizedCrop(args.image_size), transforms.RandomHorizontalFlip()]
+    if raw_uint8:
+        return t + [transforms.PILToTensor()]
+    if getattr(args, "auto_augment", None) == "ta_wide":
+        t.append(transforms.TrivialAugmentWide(interpolation=transforms.InterpolationMode.BILINEAR))
+    t += [transforms.ToTensor(), transforms.Normalize(mean=IMAGENET_MEAN, std=IMAGENET_STD)]
+    p = float(getattr(args, "random_erase", 0.0) or 0.0)
+    if p > 0:
+        t.append(transforms.RandomErasing(p=p))
+    return t
 
 
 def _limited(loader, limit: Optional[int]):
@@ -128,10 +154,14 @@ class DataPrefetcher:
     optional per-channel normalisation, casts to the compute dtype and writes channels_last - replacing the reference
     prefetcher's ``.float()``, ``sub_``, ``div_`` chain and the layout/dtype conversions the model would otherwise do.
     ``record_stream`` keeps the caching allocator from recycling a batch while the compute stream still reads it.
+
+    ``augment`` (a :class:`~..ops.augment.BatchAugment`, training batches of uint8 pixels only): each batch's draws are made
+    on the host as it is staged, copied with it, and the kernel that normalises it augments it too (``augment_normalize``;
+    a staged shard batch is first resampled to uint8 on the device).
     """
 
     def __init__(self, loader, device, dtype: torch.dtype = torch.float32, channels_last: bool = False,
-                 normalize: Optional[str] = None, limit: Optional[int] = None):
+                 normalize: Optional[str] = None, limit: Optional[int] = None, augment=None):
         self.device = torch.device(device)
         self.dtype = dtype
         self.channels_last = channels_last
@@ -149,6 +179,9 @@ class DataPrefetcher:
         self._a = torch.tensor(a, dtype=torch.float32, device=self.device)
         self._b = torch.tensor(b, dtype=torch.float32, device=self.device)
         self.identity = normalize is None
+        if augment is not None and normalize != "imagenet255":
+            raise ValueError("augmentation needs a loader of uint8 pixels")
+        self.augment = augment
         self.stream = torch.cuda.Stream(device=self.device) if self.cuda else None
 
     def __len__(self):
@@ -182,6 +215,8 @@ class DataPrefetcher:
         staged = isinstance(img, StagedBatch)
         src = img.data if staged else img
         self.h2d_bytes += src.numel() * src.element_size() + tgt.numel() * tgt.element_size()
+        if self.augment is not None:
+            return self._stage_augmented(img, src, tgt, staged)
         if not self.cuda:
             if staged:
                 raise RuntimeError("a batch staged for the device resample needs a CUDA prefetcher")
@@ -195,6 +230,31 @@ class DataPrefetcher:
                 self.loader.batch_copied(ev)
             img = self._resample(img, src) if staged else self._convert(src)
         return img, tgt
+
+    def _stage_augmented(self, img, src, tgt, staged):
+        n, _, H, W = img.shape
+        prm = self.augment.draw(n, H, W)
+        self.h2d_bytes += prm.numel() * 4
+        if not self.cuda:
+            if staged:
+                raise RuntimeError("a batch staged for the device resample needs a CUDA prefetcher")
+            return self.augment.apply(img, prm, self._a, self._b, self.dtype, self.channels_last), tgt
+        from .. import _ext
+        with torch.cuda.stream(self.stream):
+            src = src.to(self.device, non_blocking=True)
+            tgt = tgt.to(self.device, non_blocking=True)
+            prm_d = prm.to(self.device, non_blocking=True)
+            ev = torch.cuda.Event()
+            ev.record(self.stream)
+            if hasattr(self.loader, "batch_copied"):
+                self.loader.batch_copied(ev)
+            self.augment.copied(prm, ev)
+            if staged:
+                _ext.note_launch()
+                src = _ext.lib().resample_normalize(src, img.n, img.out_h, img.out_w, img.max_rows, self._a, self._b,
+                                                    _ext.lib().U8_OUT, False)
+            out = self.augment.apply(src, prm_d, self._a, self._b, self.dtype, self.channels_last)
+        return out, tgt
 
     def next(self):
         """Reference-style pull API (``data_prefetcher.next()`` in /root/reference/apex_distributed.py:160-169):
