@@ -97,6 +97,10 @@ def build_parser(entry: str = "distributed") -> argparse.ArgumentParser:
                    help="LARC clip mode: the adaptive factor is min(f / lr, 1) (default)")
     x.add_argument("--no-larc-clip", dest="larc_clip", action="store_false",
                    help="LARC scale mode: the gradient is multiplied by f itself")
+    x.add_argument("--clip-grad-norm", default=None, type=_positive_float, metavar="MAX",
+                   help="clip the unscaled, reduced gradient of every optimizer step to the global L2 norm MAX, as "
+                        "torch.nn.utils.clip_grad_norm_ (torchvision's flag); fused into the SGD step with --optimizer fused "
+                        "(default: off)")
     x.add_argument("--accum-steps", default=1, type=_positive_int, metavar="N",
                    help="gradient accumulation: one optimizer step per N consecutive batches (effective batch -b x N); the fused "
                         "engine sums the earlier passes in fp32 on each GPU and reduces once, in the last pass (default: 1)")

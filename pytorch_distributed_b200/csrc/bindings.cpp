@@ -128,6 +128,12 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("larc_sgd_multi", &larc_sgd_multi, py::arg("grads"), py::arg("params"), py::arg("momenta"), py::arg("model_copies"), py::arg("hyper"),
         py::arg("found_inf"), py::arg("nesterov"), py::arg("first"), py::arg("rows"), py::arg("stats"), py::arg("trust"), py::arg("eps"),
         py::arg("clip"), py::arg("ema") = std::vector<at::Tensor>());
+  m.def("grad_sumsq_flat", &grad_sumsq_flat, py::arg("grad"), py::arg("chunk_tensor"), py::arg("info"), py::arg("partials"),
+        py::arg("hyper"), py::arg("found_inf"));
+  m.def("grad_sumsq_multi", &grad_sumsq_multi, py::arg("grads"), py::arg("hyper"), py::arg("found_inf"), py::arg("partials"),
+        py::arg("partial_off"));
+  m.def("clip_finalize", &clip_finalize, py::arg("partials"), py::arg("nparts"), py::arg("hypers"), py::arg("clipped"), py::arg("found_inf"),
+        py::arg("total"), py::arg("count"));
   m.def("multi_tensor_scale", &multi_tensor_scale);
   m.def("multi_tensor_axpby", &multi_tensor_axpby);
   m.def("amp_update_scale", &amp_update_scale);

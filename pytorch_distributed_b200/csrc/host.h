@@ -56,6 +56,15 @@ void larc_sgd_multi(std::vector<at::Tensor> grads, std::vector<at::Tensor> param
                     std::vector<c10::optional<at::Tensor>> model_copies, at::Tensor hyper, c10::optional<at::Tensor> found_inf, bool nesterov,
                     std::vector<bool> first, std::vector<int64_t> rows, at::Tensor stats, double trust, double eps, bool clip,
                     std::vector<at::Tensor> ema);
+// Global-norm clipping: per-chunk partials of sum (g * hyper[4])^2 (flat: the LARC chunk table; multi: partials
+// [partial_off, returned value) of one buffer shared by every launch of a step), then one CTA forming the norm into `total`,
+// the clipped hyper copies (slot 4 times min(hyper[8] / (norm + 1e-6), 1)) and `count` += (coef < 1)
+void grad_sumsq_flat(at::Tensor grad, at::Tensor chunk_tensor, at::Tensor info, at::Tensor partials, at::Tensor hyper,
+                     c10::optional<at::Tensor> found_inf);
+int64_t grad_sumsq_multi(std::vector<at::Tensor> grads, at::Tensor hyper, c10::optional<at::Tensor> found_inf, at::Tensor partials,
+                         int64_t partial_off);
+void clip_finalize(at::Tensor partials, int64_t nparts, std::vector<at::Tensor> hypers, std::vector<at::Tensor> clipped,
+                   c10::optional<at::Tensor> found_inf, at::Tensor total, at::Tensor count);
 void amp_update_scale(at::Tensor scale, at::Tensor growth_tracker, at::Tensor found_inf, double growth, double backoff,
                       int64_t interval, at::Tensor hyper);
 

@@ -753,6 +753,186 @@ void larc_sgd_multi(std::vector<at::Tensor> grads, std::vector<at::Tensor> param
   });
 }
 
+// ---------------------------------------------------------------- global-norm gradient clipping (torch.nn.utils.clip_grad_norm_)
+// total = ||g * hyper[4]||_2 over every parameter of the step; coef = clamp(max_norm / (total + 1e-6), max = 1) with
+// max_norm = hyper[8] (a NaN total gives a NaN coef, an infinite one 0).  The update kernels above then run unchanged with a
+// clipped copy of each group's hyper in which slot 4 is hyper[4] * coef, so weight decay, momentum and LARC see g * coef.
+//   grad_sumsq_*   one fp32 partial sum of (g * hyper[4])^2 per chunk, over the LARC chunks (flat: its chunk table; multi:
+//                  chunks counted from each tensor's first element) and in LARC's per-chunk order;
+//   clip_finalize  one CTA: adds the partials in a fixed order, writes total, the clipped hyper copies and counts coef < 1.
+// All three return at once on found_inf, so a skipped step leaves total, the copies and the count as they were.
+// HBM traffic: the gradient once (2 B/element with a bf16 arena); the finalize reads 4 B per chunk.
+constexpr int kClipGroups = 16;
+constexpr int kClipHyperSlots = 9;  // lr, momentum, wd, dampening, gmul, momentum_pending, EMA d, EMA 1 - d, max_norm
+
+struct ClipHypers {
+  const float* src[kClipGroups];
+  float* dst[kClipGroups];
+  int32_t len[kClipGroups];
+  int32_t n;
+};
+
+// elements j < cnt of one 8-element group, in larc_acc8's order
+__device__ __forceinline__ void sumsq_acc8(const float (&g)[8], float gmul, int cnt, float& s) {
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    if (j < cnt) {
+      const float u = __fmul_rn(g[j], gmul);
+      s = __fmaf_rn(u, u, s);
+    }
+  }
+}
+
+template <typename G>
+__global__ void __launch_bounds__(kLarcThreads) grad_sumsq_flat_kernel(const G* __restrict__ grad, const int32_t* __restrict__ chunk_tensor,
+                                                                       const int64_t* __restrict__ info, float* __restrict__ partials,
+                                                                       const float* __restrict__ hyper, const int* __restrict__ found_inf) {
+  if (found_inf && *found_inf) return;
+  const int64_t q = blockIdx.x;
+  const LarcChunk k = larc_chunk(chunk_tensor, info, q);
+  const G* gp = grad + k.off + k.begin;
+  const float gmul = hyper[4];
+  float s = 0.f;
+  for (int64_t i = 8 * threadIdx.x; i < k.len; i += 8 * kLarcThreads) {
+    float g[8];
+    const int cnt = (int)min((int64_t)8, k.len - i);
+    if (cnt == 8) {
+      load8<G>(gp + i, g, /*sys=*/true);  // arena: bypass L1, as fused_sgd_flat
+    } else {
+      for (int j = 0; j < cnt; ++j) g[j] = ldcg_f(gp + i + j);
+    }
+    sumsq_acc8(g, gmul, cnt, s);
+  }
+  const float2 r = larc_cta_sum(s, 0.f);
+  if (threadIdx.x == 0) partials[q] = r.x;
+}
+
+// list 0: gradients (any float dtype); the partial of chunk c of slot t goes to partials[s.cbase[t] + c]
+__global__ void __launch_bounds__(kLarcThreads) grad_sumsq_multi_kernel(const __grid_constant__ MtaArgs<1> a, const __grid_constant__ LarcSlots s,
+                                                                        float* __restrict__ partials, const float* __restrict__ hyper,
+                                                                        const int* __restrict__ found_inf) {
+  if (found_inf && *found_inf) return;
+  const int t = a.block_tensor[blockIdx.x];
+  const int c = a.block_chunk[blockIdx.x];
+  const int64_t begin = (int64_t)c * kLarcChunk;
+  const int64_t len = min((int64_t)kLarcChunk, a.numel[t] - begin);
+  const int gdt = a.dtype[0][t];
+  const float gmul = hyper[4];
+  float acc = 0.f;
+  for (int64_t i = 8 * threadIdx.x; i < len; i += 8 * kLarcThreads) {
+    float g[8];
+    const int cnt = (int)min((int64_t)8, len - i);
+    for (int j = 0; j < cnt; ++j) g[j] = ld_any(a.ptr[0][t], gdt, begin + i + j);
+    sumsq_acc8(g, gmul, cnt, acc);
+  }
+  const float2 r = larc_cta_sum(acc, 0.f);
+  if (threadIdx.x == 0) partials[s.cbase[t] + c] = r.x;
+}
+
+// Thread i adds partials i, i + 256, ... in ascending order, then the CTA combines the thread sums in larc_cta_sum's tree.
+__global__ void __launch_bounds__(kLarcThreads) clip_finalize_kernel(const float* __restrict__ partials, int64_t nparts,
+                                                                     const __grid_constant__ ClipHypers h, const int* __restrict__ found_inf,
+                                                                     float* __restrict__ total, int* __restrict__ count) {
+  if (found_inf && *found_inf) return;
+  float s = 0.f;
+  for (int64_t i = threadIdx.x; i < nparts; i += kLarcThreads) s = __fadd_rn(s, partials[i]);
+  const float2 r = larc_cta_sum(s, 0.f);
+  __shared__ float coef_s;
+  if (threadIdx.x == 0) {
+    const float tn = __fsqrt_rn(r.x);
+    const float max_norm = h.src[0][8];
+    float coef = __fdiv_rn(max_norm, __fadd_rn(tn, 1e-6f));
+    coef = coef > 1.f ? 1.f : coef;  // torch.clamp(max=1): NaN stays NaN (fminf would return 1)
+    *total = tn;
+    if (coef < 1.f) *count += 1;
+    coef_s = coef;
+  }
+  __syncthreads();
+  const float coef = coef_s;
+  for (int g = 0; g < h.n; ++g)
+    for (int k = threadIdx.x; k < h.len[g]; k += kLarcThreads) h.dst[g][k] = k == 4 ? __fmul_rn(h.src[g][4], coef) : h.src[g][k];
+}
+
+void grad_sumsq_flat(at::Tensor grad, at::Tensor chunk_tensor, at::Tensor info, at::Tensor partials, at::Tensor hyper,
+                     c10::optional<at::Tensor> found_inf) {
+  TORCH_CHECK(grad.is_contiguous() && hyper.scalar_type() == at::kFloat && hyper.numel() >= 5, "grad_sumsq_flat: contiguous arena, fp32 hyper");
+  TORCH_CHECK(chunk_tensor.scalar_type() == at::kInt && info.scalar_type() == at::kLong && info.dim() == 2 && info.size(1) == 4 &&
+                  chunk_tensor.is_contiguous() && info.is_contiguous(), "chunk table: int32 [chunks] and int64 [tensors, 4]");
+  TORCH_CHECK(partials.scalar_type() == at::kFloat && partials.is_contiguous() && partials.numel() >= chunk_tensor.numel(),
+              "grad_sumsq_flat: fp32 partials, one per chunk");
+  const int64_t chunks = chunk_tensor.numel();
+  if (chunks == 0) return;
+  TORCH_CHECK(chunks < INT32_MAX, "too many chunks");
+  c10::cuda::CUDAGuard guard(grad.device());
+  cudaStream_t st = at::cuda::getCurrentCUDAStream();
+  const int* fi = found_inf.has_value() ? reinterpret_cast<const int*>(found_inf->data_ptr()) : nullptr;
+  const int32_t* ct = chunk_tensor.data_ptr<int32_t>();
+  const int64_t* inf = info.data_ptr<int64_t>();
+  const auto gt = grad.scalar_type();
+  auto launch = [&](auto g) {
+    using G = decltype(g);
+    grad_sumsq_flat_kernel<G><<<(int)chunks, kLarcThreads, 0, st>>>(reinterpret_cast<const G*>(grad.data_ptr()), ct, inf,
+                                                                    partials.data_ptr<float>(), hyper.data_ptr<float>(), fi);
+  };
+  if (gt == at::kBFloat16) launch(__nv_bfloat16{});
+  else if (gt == at::kHalf) launch(__half{});
+  else if (gt == at::kFloat) launch(float{});
+  else TORCH_CHECK(false, "unsupported gradient dtype");
+  C10_CUDA_KERNEL_LAUNCH_CHECK();
+}
+
+int64_t grad_sumsq_multi(std::vector<at::Tensor> grads, at::Tensor hyper, c10::optional<at::Tensor> found_inf, at::Tensor partials,
+                         int64_t partial_off) {
+  const size_t n = grads.size();
+  std::vector<int32_t> cbase(n);
+  int64_t chunks = partial_off;
+  for (size_t i = 0; i < n; ++i) {
+    cbase[i] = (int32_t)chunks;
+    chunks += (grads[i].numel() + kLarcChunk - 1) / kLarcChunk;
+  }
+  TORCH_CHECK(partial_off >= 0 && chunks < INT32_MAX, "grad_sumsq_multi: partial offset out of range");
+  TORCH_CHECK(partials.scalar_type() == at::kFloat && partials.is_contiguous() && partials.numel() >= chunks,
+              "grad_sumsq_multi: fp32 partials with room for every chunk");
+  TORCH_CHECK(hyper.scalar_type() == at::kFloat && hyper.numel() >= 5, "hyper must be fp32 with slots 0..4");
+  if (n == 0) return chunks;
+  c10::cuda::CUDAGuard guard(partials.device());
+  cudaStream_t st = at::cuda::getCurrentCUDAStream();
+  const int* fi = found_inf.has_value() ? reinterpret_cast<const int*>(found_inf->data_ptr()) : nullptr;
+  mta_for_each<1>({grads}, [&](const MtaArgs<1>& a, int nb, const int* src) {
+    LarcSlots s{};
+    for (int k = 0; k <= a.block_tensor[nb - 1]; ++k) s.cbase[k] = cbase[src[k]];
+    grad_sumsq_multi_kernel<<<nb, kLarcThreads, 0, st>>>(a, s, partials.data_ptr<float>(), hyper.data_ptr<float>(), fi);
+    C10_CUDA_KERNEL_LAUNCH_CHECK();
+  });
+  return chunks;
+}
+
+void clip_finalize(at::Tensor partials, int64_t nparts, std::vector<at::Tensor> hypers, std::vector<at::Tensor> clipped,
+                   c10::optional<at::Tensor> found_inf, at::Tensor total, at::Tensor count) {
+  TORCH_CHECK(!hypers.empty() && hypers.size() <= (size_t)kClipGroups && clipped.size() == hypers.size(),
+              "clip_finalize: 1 to ", kClipGroups, " hyper tensors, each with its clipped copy");
+  TORCH_CHECK(partials.scalar_type() == at::kFloat && partials.is_contiguous() && 0 <= nparts && nparts <= partials.numel(),
+              "clip_finalize: fp32 partials");
+  TORCH_CHECK(total.scalar_type() == at::kFloat && total.numel() >= 1 && count.scalar_type() == at::kInt && count.numel() >= 1,
+              "clip_finalize: fp32 total and int32 count");
+  ClipHypers h{};
+  for (size_t g = 0; g < hypers.size(); ++g) {
+    TORCH_CHECK(hypers[g].scalar_type() == at::kFloat && hypers[g].is_contiguous() && hypers[g].numel() >= kClipHyperSlots,
+                "clip_finalize: hyper needs slot 8 (max_norm)");
+    TORCH_CHECK(clipped[g].scalar_type() == at::kFloat && clipped[g].is_contiguous() && clipped[g].numel() == hypers[g].numel(),
+                "clip_finalize: the clipped copy must match its hyper");
+    h.src[g] = hypers[g].data_ptr<float>();
+    h.dst[g] = clipped[g].data_ptr<float>();
+    h.len[g] = (int32_t)hypers[g].numel();
+  }
+  h.n = (int32_t)hypers.size();
+  c10::cuda::CUDAGuard guard(partials.device());
+  const int* fi = found_inf.has_value() ? reinterpret_cast<const int*>(found_inf->data_ptr()) : nullptr;
+  clip_finalize_kernel<<<1, kLarcThreads, 0, at::cuda::getCurrentCUDAStream()>>>(partials.data_ptr<float>(), nparts, h, fi,
+                                                                                  total.data_ptr<float>(), count.data_ptr<int>());
+  C10_CUDA_KERNEL_LAUNCH_CHECK();
+}
+
 // Dynamic loss-scale state machine on the device (apex semantics: x2 after `interval` clean steps, /2 and skip on
 // overflow).  Also refreshes hyper[4] = grad multiplier = 1/scale, clears hyper[5] (momentum_pending) after an applied
 // step and clears found_inf for the next step.

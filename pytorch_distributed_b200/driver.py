@@ -211,6 +211,7 @@ class TrainStep:
         self.st, self.model, self.criterion, self.optimizer, self.metrics = st, model, criterion, optimizer, metrics
         self.ema = ema if ema is not None else getattr(st, "model_ema", None)   # --model-ema: once per optimizer step
         self.batch_mix = getattr(st, "batch_mix", None)
+        self.clip = getattr(st, "clip_grad_norm", None)      # --clip-grad-norm with --optimizer torch (FusedSGD clips inside)
         self.use_graph = bool(use_graph) and torch.cuda.is_available()
         self.warmup = warmup
         self.calls = 0
@@ -260,7 +261,10 @@ class TrainStep:
         if nvtx:
             torch.cuda.nvtx.range_pop()
             torch.cuda.nvtx.range_push("ptd.optimizer")
-        self.optimizer.step()
+        if self.clip is not None:
+            self.st.clip_and_step(self.optimizer, self.clip)
+        else:
+            self.optimizer.step()
         if self.ema is not None:
             self.ema.update()           # a fused optimizer has already averaged inside its step: no-op then
         if nvtx:
@@ -397,12 +401,16 @@ class Strategy:
         return model.no_sync() if hasattr(model, "no_sync") else contextlib.nullcontext()
 
     def make_optimizer(self, model, args):
+        clip = getattr(args, "clip_grad_norm", None)
+        self.clip_grad_norm = None      # --clip-grad-norm for an optimizer that does not clip inside its step (TrainStep)
         if args.optimizer == "fused":
             from .ops.fused_sgd import FusedSGD
             opt = FusedSGD(model.parameters(), args.lr, momentum=args.momentum, weight_decay=args.weight_decay,
-                           overlap_backward=bool(getattr(args, "overlap_optimizer", False)) and self.overlap_optimizer)
+                           overlap_backward=bool(getattr(args, "overlap_optimizer", False)) and self.overlap_optimizer,
+                           clip_grad_norm=clip)
         else:
             opt = torch.optim.SGD(model.parameters(), args.lr, momentum=args.momentum, weight_decay=args.weight_decay)
+            self.clip_grad_norm = clip
         if getattr(args, "larc", False):
             from .apex.parallel.LARC import LARC
             opt = LARC(opt, trust_coefficient=args.larc_trust_coefficient, clip=args.larc_clip)
@@ -445,6 +453,31 @@ class Strategy:
 
     def backward(self, loss, optimizer, last: bool = True):
         loss.backward()
+
+    def clip_and_step(self, optimizer, max_norm):
+        """``--clip-grad-norm`` with a stock optimizer: ``clip_grad_norm_`` on the reduced, unscaled ``p.grad``, then the step."""
+        self._note_clip(torch.nn.utils.clip_grad_norm_([p for g in optimizer.param_groups for p in g["params"]], max_norm), max_norm)
+        optimizer.step()
+
+    def _note_clip(self, total, max_norm):
+        """The stock path's counterpart of FusedSGD.grad_norm() / clipped_steps(), on the device (no host read per step)."""
+        if getattr(self, "clip_count", None) is None:
+            self.clip_count = torch.zeros(1, dtype=torch.int32, device=total.device)
+        self.grad_norm = total
+        self.clip_count += (max_norm / (total + 1e-6) < 1).to(torch.int32)
+
+    def clip_record(self, optimizer) -> dict:
+        """``grad_norm`` of the last clipped step and ``clipped_steps`` since the previous call, for the train JSONL record (one
+        host read each, after the epoch's synchronise)."""
+        if hasattr(optimizer, "grad_norm") and callable(optimizer.grad_norm):
+            total, count = optimizer.grad_norm(), optimizer.clipped_steps()
+        else:
+            total, count = getattr(self, "grad_norm", None), getattr(self, "clip_count", None)
+        if total is None:
+            return {"grad_norm": None, "clipped_steps": 0}
+        n = int(count.item())
+        seen, self._clipped_seen = getattr(self, "_clipped_seen", 0), n
+        return {"grad_norm": float(total.item()), "clipped_steps": n - seen}
 
     def unwrapped(self, model):
         return model.module if hasattr(model, "module") else model
@@ -540,6 +573,13 @@ class HorovodStrategy(Strategy):
         self.comm = hvd.communicator()
         self.engine = getattr(optimizer, "_ptd_engine_obj", None)
         return model, optimizer
+
+    def clip_and_step(self, optimizer, max_norm):
+        """horovod's clipping idiom: reduce, clip, then step without reducing again."""
+        optimizer.synchronize()
+        self._note_clip(torch.nn.utils.clip_grad_norm_([p for g in optimizer.param_groups for p in g["params"]], max_norm), max_norm)
+        with optimizer.skip_synchronize():
+            optimizer.step()
 
 
 class DataParallelStrategy(Strategy):
@@ -855,6 +895,8 @@ def train(train_loader, model, criterion, optimizer, epoch, st: Strategy, device
            "seconds": time.time() - t0, "loss": losses.avg, "acc1": top1.avg, "acc5": top5.avg}
     if accum > 1:
         rec.update(accum_steps=accum, optimizer_steps=n_batches // accum)
+    if getattr(args, "clip_grad_norm", None) is not None:
+        rec.update(st.clip_record(optimizer))
     _log_jsonl(args, rec)
     return losses.avg
 

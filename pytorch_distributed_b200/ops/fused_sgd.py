@@ -16,9 +16,17 @@ update pass per flat step, per bucket in overlap mode, or per group in multi-ten
 ``attach_ema`` (what :class:`~pytorch_distributed_b200.utils.ema.ModelEma` calls) folds an exponential moving average of
 the fp32 masters into the update kernels of every mode (one more fp32 read and write per element), and averages the
 model's float buffers with one ``ema_multi`` launch at the end of each step.  The decay sits in hyper slots 6 and 7.
+
+``clip_grad_norm`` / ``set_clip_grad_norm`` (``--clip-grad-norm``) clip the unscaled, reduced gradient to a global L2 norm, as
+``torch.nn.utils.clip_grad_norm_`` right before the step: a norm pass over every gradient of the step, then one CTA that
+writes a clipped copy of each group's hyper tensor (slot 4, the gradient multiplier, times the clip coefficient), which the
+unchanged update kernels take in place of ``hyper``.  ``max_norm`` sits in hyper slot 8.  While clipping is on, the
+per-bucket update of overlap mode stays off: no bucket may be updated before the last gradient is known.
 """
 from __future__ import annotations
 
+import math
+from types import SimpleNamespace
 from typing import Optional
 
 import torch
@@ -57,7 +65,7 @@ def larc_reference_grad(p, g, lr, weight_decay, trust_coefficient, clip, eps):
 
 class FusedSGD(Optimizer):
     def __init__(self, params, lr=0.1, momentum=0.0, dampening=0.0, weight_decay=0.0, nesterov=False, flat: Optional[bool] = None,
-                 overlap_backward: bool = False):
+                 overlap_backward: bool = False, clip_grad_norm: Optional[float] = None):
         if nesterov and (momentum <= 0 or dampening != 0):
             raise ValueError("Nesterov momentum requires a momentum and zero dampening")
         defaults = dict(lr=lr, momentum=momentum, dampening=dampening, weight_decay=weight_decay, nesterov=nesterov)
@@ -82,6 +90,9 @@ class FusedSGD(Optimizer):
         self._larc_tab = None       # flat mode: chunk table of the arena layout (built once)
         self._ema = None            # ModelEma updated inside the step (attach_ema)
         self._ema_flat = None       # flat mode: its parameter averages in the arena layout
+        self._clip = None           # max_norm of global-norm gradient clipping (set_clip_grad_norm)
+        self._clip_state = None     # norm, clipped-step count, clipped hyper copies, partials (made by the first clipped step)
+        self.set_clip_grad_norm(clip_grad_norm)
         self._try_bind()
 
     # ------------------------------------------------------------------ engine binding (flat mode)
@@ -117,7 +128,7 @@ class FusedSGD(Optimizer):
                                "engine's fp32_grad_accumulation=True and no_sync() (--accum-steps), which keeps the per-bucket "
                                "update, or use overlap_backward=False (--no-overlap-optimizer)")
         self._ov_applied = 0
-        self._ov_active = self._flat is not None and self._amp is None
+        self._ov_active = self._flat is not None and self._amp is None and self._clip is None
         if self._ov_active:
             self._ov_first = self._steps == 0
             self._hyper_tensor(0, self.param_groups[0], self._flat.master.device)
@@ -251,6 +262,98 @@ class FusedSGD(Optimizer):
         _ext.note_launch()
         _ext.lib().ema_multi(live, shadow, hyper[6:8], found_inf)
 
+    # ------------------------------------------------------------------ global-norm gradient clipping (clip_grad_norm_)
+    def set_clip_grad_norm(self, max_norm: Optional[float]) -> None:
+        """Clip the unscaled gradient of every following step to the global L2 norm ``max_norm`` (None: no clipping).  A step
+        captured in a CUDA graph follows a new value on replay; turning clipping on or off takes a new capture."""
+        if max_norm is not None:
+            max_norm = float(max_norm)
+            if not (max_norm > 0 and math.isfinite(max_norm)):
+                raise ValueError("clip_grad_norm needs a positive finite max_norm, got %r" % (max_norm,))
+        self._clip = max_norm
+        self.refresh_hyper()
+
+    def grad_norm(self) -> Optional[torch.Tensor]:
+        """fp32 scalar tensor: the global norm of the unscaled gradient before clipping, as of the last applied clipped step
+        (what ``clip_grad_norm_`` returns); None before the first clipped step."""
+        return self._clip_state.total if self._clip_state is not None else None
+
+    def clipped_steps(self) -> Optional[torch.Tensor]:
+        """int32 tensor of one element: the number of applied steps whose clip coefficient was below 1; None before the
+        first clipped step."""
+        return self._clip_state.count if self._clip_state is not None else None
+
+    def _clip_on(self, device):
+        if self._clip_state is None:
+            self._clip_state = SimpleNamespace(total=torch.zeros((), dtype=torch.float32, device=device),
+                                               count=torch.zeros(1, dtype=torch.int32, device=device), hyper={}, partials=None)
+        return self._clip_state
+
+    def _clipped_copy(self, gi, hyper):
+        cs = self._clip_on(hyper.device)
+        t = cs.hyper.get(gi)
+        if t is None or t.numel() != hyper.numel():
+            t = cs.hyper[gi] = torch.zeros_like(hyper)
+        return t
+
+    def _clip_flat(self, hyper, found_inf):
+        """Norm pass over the arena's parameter ranges and finalize; returns the clipped copy of ``hyper``."""
+        fs, tab = self._flat, self._larc_table()
+        cs = self._clip_on(hyper.device)
+        clipped = self._clipped_copy(0, hyper)
+        from .. import _ext
+        _ext.note_launch(2)
+        _ext.lib().grad_sumsq_flat(fs.engine.grad_arena(), tab.chunk_tensor, tab.info, tab.partials, hyper, found_inf)
+        _ext.lib().clip_finalize(tab.partials, tab.chunks, [hyper], [clipped], found_inf, cs.total, cs.count)
+        return clipped
+
+    @staticmethod
+    def _kernel_group(params) -> bool:
+        return params[0].is_cuda and all(p.dtype in (torch.float32, torch.bfloat16, torch.float16) for p in params)
+
+    def _clip_multi(self, amp):
+        """Multi-tensor and PyTorch modes: the clipping of this step, over every group.  Returns ``{group index: clipped
+        hyper}`` on the kernel path, the clip coefficient (a 0-d tensor) on the PyTorch path, None when nothing is clipped."""
+        groups = [(gi, [p for p in g["params"] if p.grad is not None]) for gi, g in enumerate(self.param_groups)]
+        groups = [(gi, ps) for gi, ps in groups if ps]
+        if not groups:
+            return None
+        kinds = {self._kernel_group(ps) for _, ps in groups}
+        if len(kinds) != 1:
+            raise NotImplementedError("clip_grad_norm: the parameter groups mix the CUDA kernels and the PyTorch path")
+        if kinds.pop():
+            from .. import _ext
+            C = _ext.lib()
+            dev = groups[0][1][0].device
+            cs = self._clip_on(dev)
+            need = sum(-(-p.numel() // C.LARC_CHUNK) for _, ps in groups for p in ps)
+            if cs.partials is None or cs.partials.numel() < need:
+                cs.partials = torch.zeros(max(need, 1), dtype=torch.float32, device=dev)
+            fi = amp.found_inf if amp is not None else None
+            hypers, off = [], 0
+            for gi, ps in groups:
+                hyper = self._hyper_tensor(gi, self.param_groups[gi], dev)
+                if amp is not None:
+                    amp.attach_hyper(hyper)
+                hypers.append(hyper)
+                _ext.note_launch()
+                off = C.grad_sumsq_multi([p.grad for p in ps], hyper, fi, cs.partials, off)
+            clipped = [self._clipped_copy(gi, h) for (gi, _), h in zip(groups, hypers)]
+            _ext.note_launch()
+            C.clip_finalize(cs.partials, off, hypers, clipped, fi, cs.total, cs.count)
+            return {gi: c for (gi, _), c in zip(groups, clipped)}
+        if amp is not None and amp.host_found_inf():
+            return None
+        gmul = amp.host_inv_scale() if amp is not None else 1.0
+        grads = [p.grad if gmul == 1.0 else p.grad.float() * gmul for _, ps in groups for p in ps]
+        # torch.nn.utils.clip_grad_norm_'s arithmetic (L2, foreach) on the unscaled gradients, which stay unwritten in p.grad
+        total = torch.nn.utils.get_total_norm(grads, 2.0)
+        coef = torch.clamp(self._clip / (total + 1e-6), max=1.0)
+        cs = self._clip_on(total.device)
+        cs.total.copy_(total)
+        cs.count.add_((coef < 1).to(cs.count.dtype))
+        return coef
+
     @property
     def is_flat(self) -> bool:
         return self._flat is not None
@@ -260,13 +363,14 @@ class FusedSGD(Optimizer):
         gmul = 1.0
         vals = (float(group["lr"]), float(group["momentum"]), float(group["weight_decay"]), float(group["dampening"]))
         dw = self._ema.decay_pair() if self._ema is not None else (0.0, 0.0)      # slots 6, 7: EMA decay d and fp32(1 - d)
+        clip = self._clip if self._clip is not None else 0.0                       # slot 8: max_norm of gradient clipping
         ent = self._hyper.get(gi)
         if ent is None:
             # slot 5 (momentum_pending): under dynamic loss scaling the momentum is initialised by the first step that is
             # actually applied; the loss scaler clears the slot after it (csrc/optim.cu)
             pending = 1.0 if self._steps == 0 else 0.0
-            t = torch.tensor(list(vals) + [gmul, pending] + list(dw), dtype=torch.float32, device=device)
-            self._hyper[gi] = [t, vals, dw]
+            t = torch.tensor(list(vals) + [gmul, pending] + list(dw) + [clip], dtype=torch.float32, device=device)
+            self._hyper[gi] = [t, vals, dw, clip]
             return t
         if ent[1] != vals:
             # only lr..dampening and the EMA slots are host-owned; slot 4 (gradient multiplier) belongs to the loss scaler kernel
@@ -275,10 +379,13 @@ class FusedSGD(Optimizer):
         if ent[2] != dw:
             ent[0][6:8].copy_(torch.tensor(dw, dtype=torch.float32), non_blocking=True)
             ent[2] = dw
+        if ent[3] != clip:
+            ent[0][8:9].fill_(clip)
+            ent[3] = clip
         return ent[0]
 
     def refresh_hyper(self) -> None:
-        """Push changed lr/momentum/weight-decay to the device copies (needed when ``step`` is replayed from a CUDA graph)."""
+        """Push changed lr/momentum/weight-decay/max_norm to the device copies (needed when ``step`` is replayed from a CUDA graph)."""
         for gi, ent in self._hyper.items():
             self._hyper_tensor(gi, self.param_groups[gi], ent[0].device)
 
@@ -312,19 +419,21 @@ class FusedSGD(Optimizer):
             if amp is not None:
                 amp.attach_hyper(hyper)
             from .. import _ext
+            step_hyper = self._clip_flat(hyper, amp.found_inf if amp is not None else None) if self._clip is not None else hyper
             if self._larc is not None:
-                self._larc_flat(hyper, amp.found_inf if amp is not None else None, first)
+                self._larc_flat(step_hyper, amp.found_inf if amp is not None else None, first)
             else:
                 _ext.note_launch()
-                _ext.lib().fused_sgd_flat(fs.engine.grad_arena(), fs.master, fs.momentum, fs.model_copy, hyper,
+                _ext.lib().fused_sgd_flat(fs.engine.grad_arena(), fs.master, fs.momentum, fs.model_copy, step_hyper,
                                           amp.found_inf if amp is not None else None, bool(group["nesterov"]), first,
                                           ema=self._ema_flat)
             self._ema_buffers(hyper, amp.found_inf if amp is not None else None)
             if amp is not None:
                 amp.update()
         else:
+            clipped = self._clip_multi(amp) if self._clip is not None else None
             for gi, group in enumerate(self.param_groups):
-                self._step_group(gi, group, first, amp)
+                self._step_group(gi, group, first, amp, clipped)
             self._ema_buffers_multi(amp)
             if amp is not None:
                 amp.update()
@@ -344,7 +453,8 @@ class FusedSGD(Optimizer):
                 raise RuntimeError("FusedSGD.step(): the gradient engine holds accumulated no_sync() passes that no synchronising "
                                    "backward has reduced yet - run the last micro-batch's backward outside no_sync() first")
 
-    def _step_group(self, gi, group, first, amp):
+    def _step_group(self, gi, group, first, amp, clipped=None):
+        """``clipped``: what ``_clip_multi`` returned for this step (clipped hyper copies, or the PyTorch path's coefficient)."""
         params = [p for p in group["params"] if p.grad is not None]
         if not params:
             return
@@ -355,12 +465,14 @@ class FusedSGD(Optimizer):
                 st["momentum_buffer"] = torch.zeros_like(p, dtype=torch.float32, memory_format=torch.preserve_format)
                 st["_fresh"] = True
             bufs.append(st["momentum_buffer"])
-        if params[0].is_cuda and all(p.dtype in (torch.float32, torch.bfloat16, torch.float16) for p in params):
+        if self._kernel_group(params):
             from .. import _ext
             C = _ext.lib()
             hyper = self._hyper_tensor(gi, group, params[0].device)
             if amp is not None:
                 amp.attach_hyper(hyper)
+            if clipped is not None:
+                hyper = clipped[gi]
             fresh = [p for p in params if self.state[p].pop("_fresh", False)]
 
             def master_of(p):
@@ -407,6 +519,8 @@ class FusedSGD(Optimizer):
             for p, buf in zip(params, bufs):
                 fresh = self.state[p].pop("_fresh", False)
                 g = p.grad if gmul == 1.0 else p.grad.float() * gmul
+                if clipped is not None:
+                    g = g * clipped
                 st = self.state[p]
                 if p.dtype != torch.float32 and "master" not in st:
                     st["master"] = p.detach().float().clone()

@@ -561,6 +561,7 @@ def DistributedOptimizer(optimizer, named_parameters=None, compression=Compressi
     engine = _FusionEngine(named_parameters, comm, wire, thr, cyc, backward_passes_per_step)
 
     base = optimizer.__class__
+    skip = [False]                      # inside skip_synchronize(): step() after an explicit synchronize() does not wait again
 
     class _DistributedOptimizer(base):  # type: ignore[misc,valid-type]
         def __init__(self):             # state is shared with the wrapped instance, not re-created
@@ -570,12 +571,23 @@ def DistributedOptimizer(optimizer, named_parameters=None, compression=Compressi
             engine.synchronize()
 
         def step(self, closure=None):
-            engine.synchronize()
+            if not skip[0]:
+                engine.synchronize()
             return base.step(self, closure) if closure is not None else base.step(self)
 
         def skip_synchronize(self):
+            """horovod's ``with optimizer.skip_synchronize(): optimizer.step()`` after ``optimizer.synchronize()`` and gradient
+            surgery (clipping): the step does not synchronise a second time, which would count a second step in the autotuner."""
             import contextlib
-            return contextlib.nullcontext()
+
+            @contextlib.contextmanager
+            def ctx():
+                skip[0] = True
+                try:
+                    yield
+                finally:
+                    skip[0] = False
+            return ctx()
 
     wrapped = _DistributedOptimizer.__new__(_DistributedOptimizer)
     wrapped.__dict__ = optimizer.__dict__

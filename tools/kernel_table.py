@@ -38,6 +38,14 @@ KERNELS = [
      "LARC update: trust ratio from the chunk partials + SGD momentum + bf16 copy + statistics", "tests/test_gpu_larc.py, tools/larc_bench.py"),
     (r"larc_norm_multi_kernel", "larc_norm_multi_kernel", "optim.cu", "LARC norm pass, multi-tensor-apply variant", "tests/test_gpu_larc.py"),
     (r"larc_sgd_multi_kernel", "larc_sgd_multi_kernel", "optim.cu", "LARC update, multi-tensor-apply variant", "tests/test_gpu_larc.py"),
+    (r"grad_sumsq_flat_kernelI13__nv_bfloat16E", "grad_sumsq_flat_kernel<bf16>", "optim.cu",
+     "--clip-grad-norm norm pass: per-chunk fp32 sums of (g gmul)^2 over the arena's parameter ranges, LARC's order",
+     "tests/test_gpu_clip_grad_norm.py, tools/clip_bench.py"),
+    (r"grad_sumsq_multi_kernel", "grad_sumsq_multi_kernel", "optim.cu", "--clip-grad-norm norm pass, multi-tensor-apply variant",
+     "tests/test_gpu_clip_grad_norm.py"),
+    (r"clip_finalize_kernel", "clip_finalize_kernel", "optim.cu",
+     "--clip-grad-norm: one CTA adds the partials in a fixed order, writes the norm, the clipped hyper copies and the count",
+     "tests/test_gpu_clip_grad_norm.py, tools/clip_bench.py"),
     (r"multi_tensor_scale_kernel", "multi_tensor_scale_kernel", "optim.cu", "amp unscale with non-finite flag", "tests/test_gpu_kernels.py"),
     (r"amp_update_scale_kernel", "amp_update_scale_kernel", "optim.cu", "loss-scale state machine on the device", "tests/test_gpu_kernels.py"),
     (r"bn_stats_kernelI13__nv_bfloat16E", "bn_stats_kernel<bf16>", "bn_act.cu", "BN forward statistics (one row of partial sums per CTA)", "tests/test_gpu_kernels.py"),
