@@ -118,9 +118,10 @@ def build_parser(entry: str = "distributed") -> argparse.ArgumentParser:
     x.add_argument("--cutmix-alpha", default=0.0, type=_alpha, metavar="A",
                    help="CutMix with lambda ~ Beta(A, A), as torchvision's transforms.v2.CutMix; with --mixup-alpha too, each "
                         "batch takes one of the two at random (default: 0.0 = off)")
-    x.add_argument("--auto-augment", default=None, choices=["ta_wide"],
-                   help="per-sample TrivialAugment Wide on the training crops, as torchvision's transforms.v2.TrivialAugmentWide "
-                        "(bilinear); fused into the normalising kernel on the GPU (default: none)")
+    x.add_argument("--auto-augment", default=None, choices=["ta_wide", "imagenet", "cifar10", "svhn"],
+                   help="per-sample augmentation of the training crops: ta_wide is torchvision's transforms.v2.TrivialAugmentWide, "
+                        "imagenet, cifar10 and svhn are transforms.v2.AutoAugment with that policy (all bilinear); fused into "
+                        "the normalising kernel on the GPU (default: none)")
     x.add_argument("--random-erase", default=0.0, type=_unit_float, metavar="P",
                    help="erase a random box of each training image with probability P, as torchvision's RandomErasing(P) after "
                         "the normalisation (default: 0.0)")

@@ -1,6 +1,6 @@
 // Per-sample input augmentation of a uint8 batch, fused with the normalise / cast / layout pass of normalize_kernel
-// (data_ops.cu): torchvision's transforms.v2.TrivialAugmentWide(interpolation=BILINEAR) on the uint8 image, then the
-// normalisation, then RandomErasing(value=0) on the normalised tensor.
+// (data_ops.cu): torchvision's transforms.v2.TrivialAugmentWide or AutoAugment(interpolation=BILINEAR) on the uint8 image,
+// then the normalisation, then RandomErasing(value=0) on the normalised tensor.
 //
 //  augment_normalize : one CTA per sample.  An op that needs a per-image statistic first reduces it inside the CTA in
 //                      integers (no float atomics, so the result does not depend on the order of the threads), then one
@@ -8,13 +8,21 @@
 //                      normalises them with the single FMA of normalize_nhwc / resample_normalize and zeroes the erase box
 //                      in the same store.  Geometric ops gather their four taps from global memory (the sample, 150 KB
 //                      at 224^2, stays in L2).
+//                      A two-op table (AutoAugment's sub-policies) takes two launches: augment_stage_kernel writes op A's
+//                      uint8 output into a scratch batch, then augment_chain_kernel runs op B on it as above (on the
+//                      source for a row whose op A is Identity, i.e. not applied).  Measured on the H100, this beat one
+//                      pass with op A's output in shared memory (3 H W bytes per CTA leave one CTA per SM).
 //
-// The host draws every sample's op and magnitude and encodes what the kernel needs into a row of prm [n, kAugPrm] float32
-// (pytorch_distributed_b200/ops/augment.py):
-//   prm[0]     kernel op (AugOp below; anything else copies the image)
-//   prm[1..6]  op parameters (below)
-//   prm[7]     1: erase rows [prm[8], prm[8] + prm[10]) x columns [prm[9], prm[9] + prm[11])
-//   prm[12..]  not read here (the policy's op index and signed magnitude, for the CPU reference)
+// The host draws every sample's ops and magnitudes and encodes what the kernel needs into a row of prm float32
+// (pytorch_distributed_b200/ops/augment.py), [n, kAugPrm] for one op per sample or [n, kAugChainPrm] for two:
+//   prm[0]      op A's kernel code (AugOp below; anything else copies the image)
+//   prm[1..6]   op A's parameters (below)
+//   prm[7]      1: erase rows [prm[8], prm[8] + prm[10]) x columns [prm[9], prm[9] + prm[11])
+//   prm[12..15] not read here (op A's index into op_names() + ("Invert",) and its signed magnitude, for the CPU reference)
+//   prm[16]     two-op rows only: op B's kernel code, applied to op A's output
+//   prm[17..22] op B's parameters
+//   prm[23..31] not read here (op B's index and signed magnitude in prm[23], prm[24], for the CPU reference)
+// kInvert exists in two-op rows only: in a one-op row it is an unknown code, and the one-op kernel is unchanged by it.
 //
 // Float order.  Every rounding torchvision's CPU kernels make is written out with __fmul_rn / __fadd_rn / __fmaf_rn /
 // __fdiv_rn (the extension builds with --use_fast_math, which would contract products into FMAs and make `/` approximate):
@@ -49,7 +57,10 @@ enum AugOp : int {
   kSolarize = 8,     // prm[1]: fp32 threshold
   kAutoContrast = 9,
   kEqualize = 10,
+  kInvert = 11,      // 255 - v (two-op rows only)
 };
+
+constexpr int kColB = 16;   // first column of op B in a two-op row
 
 constexpr int kThreads = 512;
 
@@ -78,24 +89,22 @@ __device__ __forceinline__ int bilinear(const uint8_t* p, int H, int W, float ix
   return (int)fminf(255.f, fmaxf(0.f, rintf(v)));
 }
 
-template <typename Out, bool NHWC_OUT>
-__global__ void __launch_bounds__(kThreads) augment_normalize_kernel(const uint8_t* __restrict__ src, Out* __restrict__ dst,
-                                                                    const float* __restrict__ prm, int prm_stride,
-                                                                    const float* __restrict__ na, const float* __restrict__ nb,
-                                                                    int H, int W) {
-  __shared__ int hist[3][256];
-  __shared__ int lut[3][256];
-  __shared__ int red[6];                   // Contrast: [0] sum; AutoContrast: [0..2] min, [3..5] max
-  const int s = blockIdx.x;
+// One op over one sample: its per-image statistic (integer, order-free), then one streaming pass over the output pixels.
+// src + k: the sample's three planes; q: the op's columns (q[0] kernel code, q[1..6] parameters);
+// row: the sample's row (erase box).  kChain: the two-op kernel, which also knows kInvert.  kStage: write the op's uint8
+// result to stage (the sample's three planes in the scratch batch) instead of erasing, normalising and storing it.
+template <typename Out, bool NHWC_OUT, bool kChain, bool kStage>
+__device__ __forceinline__ void apply_op(const uint8_t* src, int k, const float* q, const float* row, Out* dst, uint8_t* stage,
+                                         int s, int H, int W, const float* na, const float* nb, int (*hist)[256], int (*lut)[256],
+                                         int* red) {
   const int HW = H * W;
   const size_t plane = (size_t)HW;
-  const uint8_t* img = src + (size_t)s * 3 * plane;
-  const float* q = prm + (size_t)s * prm_stride;
+  const uint8_t* img = src + (size_t)k * 3 * plane;
   const int op = (int)q[0];
   const float p1 = q[1], p2 = q[2];
   const float sa[3] = {na[0], na[1], na[2]}, sb[3] = {nb[0], nb[1], nb[2]};
-  const bool erase = q[7] != 0.f;
-  const int ei = (int)q[8], ej = (int)q[9], eh = (int)q[10], ew = (int)q[11];
+  const bool erase = row[7] != 0.f;
+  const int ei = (int)row[8], ej = (int)row[9], eh = (int)row[10], ew = (int)row[11];
 
   // ---- per-image statistics (integer, order-free)
   if (op == kContrast || op == kAutoContrast || op == kEqualize) {
@@ -215,7 +224,18 @@ __global__ void __launch_bounds__(kThreads) augment_normalize_kernel(const uint8
         for (int c = 0; c < 3; ++c) v[c] = lut[c][v[c]];
         break;
       default:
+        if constexpr (kChain) {
+          if (op == kInvert) {
+#pragma unroll
+            for (int c = 0; c < 3; ++c) v[c] = 255 - v[c];
+          }
+        }
         break;
+    }
+    if constexpr (kStage) {
+#pragma unroll
+      for (int c = 0; c < 3; ++c) stage[c * plane + p] = (uint8_t)v[c];
+      continue;
     }
     const bool zero = erase && y >= ei && y < ei + eh && x >= ej && x < ej + ew;
     float o[3];
@@ -233,13 +253,65 @@ __global__ void __launch_bounds__(kThreads) augment_normalize_kernel(const uint8
   }
 }
 
+// one op per sample: prm [n, kAugPrm]
+template <typename Out, bool NHWC_OUT>
+__global__ void __launch_bounds__(kThreads) augment_normalize_kernel(const uint8_t* __restrict__ src, Out* __restrict__ dst,
+                                                                    const float* __restrict__ prm, int prm_stride,
+                                                                    const float* __restrict__ na, const float* __restrict__ nb,
+                                                                    int H, int W) {
+  __shared__ int hist[3][256];
+  __shared__ int lut[3][256];
+  __shared__ int red[6];                   // Contrast: [0] sum; AutoContrast: [0..2] min, [3..5] max
+  const int s = blockIdx.x;
+  const float* q = prm + (size_t)s * prm_stride;
+  apply_op<Out, NHWC_OUT, false, false>(src, s, q, q, dst, nullptr, s, H, W, na, nb, hist, lut, red);
+}
+
+// two ops per sample, launch 1: op A of each sample that applies it, into the uint8 scratch batch
+__global__ void __launch_bounds__(kThreads) augment_stage_kernel(const uint8_t* __restrict__ src, uint8_t* __restrict__ scratch,
+                                                                const float* __restrict__ prm, int H, int W) {
+  __shared__ int hist[3][256];
+  __shared__ int lut[3][256];
+  __shared__ int red[6];
+  const int s = blockIdx.x;
+  const float* q = prm + (size_t)s * kAugChainPrm;
+  if ((int)q[0] == kIdentity) return;      // op A not applied: launch 2 reads the source
+  // the normalisation is not read by a stage; q stands in for its pointers
+  apply_op<float, false, true, true>(src, s, q, q, nullptr, scratch + (size_t)s * 3 * H * W, s, H, W, q, q, hist, lut, red);
+}
+
+// two ops per sample, launch 2: op B on op A's output (the source where op A is not applied), erase, normalise, store
+template <typename Out, bool NHWC_OUT>
+__global__ void __launch_bounds__(kThreads) augment_chain_kernel(const uint8_t* __restrict__ src, const uint8_t* __restrict__ scratch,
+                                                                Out* __restrict__ dst, const float* __restrict__ prm,
+                                                                const float* __restrict__ na, const float* __restrict__ nb, int H,
+                                                                int W) {
+  __shared__ int hist[3][256];
+  __shared__ int lut[3][256];
+  __shared__ int red[6];
+  const int s = blockIdx.x;
+  const float* q = prm + (size_t)s * kAugChainPrm;
+  const uint8_t* from = (int)q[0] == kIdentity ? src : scratch;
+  apply_op<Out, NHWC_OUT, true, false>(from, s, q + kColB, q, dst, nullptr, s, H, W, na, nb, hist, lut, red);
+}
+
 template <typename Out>
 void launch(const at::Tensor& src, at::Tensor& dst, const at::Tensor& prm, const at::Tensor& a, const at::Tensor& b, bool nhwc) {
   const int n = (int)src.size(0), H = (int)src.size(2), W = (int)src.size(3);
-  auto kernel = nhwc ? augment_normalize_kernel<Out, true> : augment_normalize_kernel<Out, false>;
-  kernel<<<n, kThreads, 0, at::cuda::getCurrentCUDAStream()>>>(src.data_ptr<uint8_t>(), reinterpret_cast<Out*>(dst.data_ptr()),
-                                                               prm.data_ptr<float>(), (int)prm.size(1), a.data_ptr<float>(),
-                                                               b.data_ptr<float>(), H, W);
+  const cudaStream_t stream = at::cuda::getCurrentCUDAStream();
+  if (prm.size(1) == kAugChainPrm) {
+    at::Tensor scratch = at::empty_like(src);
+    augment_stage_kernel<<<n, kThreads, 0, stream>>>(src.data_ptr<uint8_t>(), scratch.data_ptr<uint8_t>(), prm.data_ptr<float>(),
+                                                     H, W);
+    C10_CUDA_KERNEL_LAUNCH_CHECK();
+    auto kernel = nhwc ? augment_chain_kernel<Out, true> : augment_chain_kernel<Out, false>;
+    kernel<<<n, kThreads, 0, stream>>>(src.data_ptr<uint8_t>(), scratch.data_ptr<uint8_t>(), reinterpret_cast<Out*>(dst.data_ptr()),
+                                       prm.data_ptr<float>(), a.data_ptr<float>(), b.data_ptr<float>(), H, W);
+  } else {
+    auto kernel = nhwc ? augment_normalize_kernel<Out, true> : augment_normalize_kernel<Out, false>;
+    kernel<<<n, kThreads, 0, stream>>>(src.data_ptr<uint8_t>(), reinterpret_cast<Out*>(dst.data_ptr()), prm.data_ptr<float>(),
+                                       (int)prm.size(1), a.data_ptr<float>(), b.data_ptr<float>(), H, W);
+  }
   C10_CUDA_KERNEL_LAUNCH_CHECK();
 }
 
@@ -254,8 +326,9 @@ at::Tensor augment_normalize(const at::Tensor& src, const at::Tensor& prm, const
   TORCH_CHECK(H * W <= kAugMaxPixels, "augment_normalize: images of more than 65793 pixels (kAugMaxPixels), beyond which "
               "Contrast's float32 mean is no longer exact in torchvision's order");
   TORCH_CHECK(prm.device() == src.device() && prm.scalar_type() == at::kFloat && prm.is_contiguous() && prm.dim() == 2 &&
-                  prm.size(0) == n && prm.size(1) == kAugPrm,
-              "augment_normalize: prm must be a contiguous float32 [n, kAugPrm] tensor on the batch's device");
+                  prm.size(0) == n && (prm.size(1) == kAugPrm || prm.size(1) == kAugChainPrm),
+              "augment_normalize: prm must be a contiguous float32 [n, kAugPrm] (one op per sample) or [n, kAugChainPrm] "
+              "(two) tensor on the batch's device");
   TORCH_CHECK(a.scalar_type() == at::kFloat && b.scalar_type() == at::kFloat && a.numel() == 3 && b.numel() == 3 &&
                   a.device() == src.device() && b.device() == src.device(),
               "augment_normalize: a and b must be float32 [3] on the batch's device");

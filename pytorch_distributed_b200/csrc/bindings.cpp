@@ -163,6 +163,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("augment_normalize", &augment_normalize, py::arg("src"), py::arg("prm"), py::arg("a"), py::arg("b"), py::arg("out_dtype"),
         py::arg("channels_last"));
   m.attr("AUG_PRM") = kAugPrm;
+  m.attr("AUG_CHAIN_PRM") = kAugChainPrm;
   m.attr("AUG_MAX_PIXELS") = kAugMaxPixels;
   m.def("p2p_copy_multi", &p2p_copy_multi);
   m.def("mix_batch", &mix_batch, py::arg("x"), py::arg("out"), py::arg("y"), py::arg("yb"), py::arg("dom"), py::arg("prm"));

@@ -143,9 +143,11 @@ std::vector<at::Tensor> soft_ce_fwd(const at::Tensor& z, const at::Tensor& ya, c
 at::Tensor soft_ce_bwd(const at::Tensor& z, const at::Tensor& ya, const at::Tensor& yb, const at::Tensor& prm, const at::Tensor& lse,
                        const at::Tensor& g, double eps);
 
-// ---- augment.cu (prm: float32 [n, kAugPrm], one row of encoded op parameters per sample, see augment.cu)
-// TrivialAugmentWide + normalise + RandomErasing of a uint8 NCHW batch; returns what normalize_nhwc returns for it unaugmented
-constexpr int64_t kAugPrm = 16;
+// ---- augment.cu (prm: float32 [n, kAugPrm] or [n, kAugChainPrm], one row of encoded op parameters per sample, see augment.cu)
+// TrivialAugmentWide or AutoAugment + normalise + RandomErasing of a uint8 NCHW batch; returns what normalize_nhwc returns for
+// it unaugmented
+constexpr int64_t kAugPrm = 16;               // one op per sample
+constexpr int64_t kAugChainPrm = 32;          // two ops per sample, the second applied to the first's output
 constexpr int64_t kAugMaxPixels = 65793;      // 255 H W < 2^24: Contrast's float32 grayscale sum is exact in any order
 at::Tensor augment_normalize(const at::Tensor& src, const at::Tensor& prm, const at::Tensor& a, const at::Tensor& b, int64_t out_dtype,
                              bool channels_last);

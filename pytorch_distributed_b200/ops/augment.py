@@ -1,12 +1,16 @@
-"""TrivialAugment Wide and random erasing of training batches (``--auto-augment ta_wide``, ``--random-erase P``).
+"""TrivialAugment Wide, AutoAugment and random erasing of training batches (``--auto-augment ta_wide|imagenet|cifar10|svhn``,
+``--random-erase P``).
 
 The semantics are torchvision 0.26's, applied per sample as the classification recipe's ``ClassificationPresetTrain`` does:
-``transforms.v2.TrivialAugmentWide(interpolation=BILINEAR)`` on the uint8 crop, then the normalisation, then
-``transforms.v2.RandomErasing(p, scale=(0.02, 0.33), ratio=(0.3, 3.3), value=0)`` on the normalised tensor.
+``transforms.v2.TrivialAugmentWide(interpolation=BILINEAR)`` or ``transforms.v2.AutoAugment(policy, interpolation=BILINEAR)``
+on the uint8 crop, then the normalisation, then ``transforms.v2.RandomErasing(p, scale=(0.02, 0.33), ratio=(0.3, 3.3),
+value=0)`` on the normalised tensor.
 
-On the GPU one ``augment_normalize`` launch (``csrc/augment.cu``) does all three for the whole batch and returns what
-``normalize_nhwc`` returns: the draws of a batch are encoded on the host into a pinned ``[n, AUG_PRM]`` float32 table that
-travels to the device with the batch.  On the CPU, :meth:`BatchAugment.reference_apply` runs torchvision's own functional ops
+On the GPU one ``augment_normalize`` call (``csrc/augment.cu``; two launches for two ops) does all three for the whole batch
+and returns what ``normalize_nhwc`` returns: the draws of a batch are encoded on the host into a pinned float32 table that
+travels to the device with the batch, ``[n, AUG_PRM]`` for TrivialAugment Wide's one op per sample and ``[n, AUG_CHAIN_PRM]``
+for an AutoAugment sub-policy's two ops, the second applied to the first's output.  On the CPU,
+:meth:`BatchAugment.reference_apply` runs torchvision's own functional ops
 per sample; it is also the reference of the GPU tests.
 """
 from __future__ import annotations
@@ -19,6 +23,10 @@ import numpy as np
 import torch
 
 AUG_PRM = 16                    # columns of the parameter table (kAugPrm in csrc/host.h)
+AUG_CHAIN_PRM = 32              # columns of a two-op table (kAugChainPrm): op B's code and parameters in 16..22
+COL_B = 16                      # op B's first column; its op index and signed magnitude are in COL_B + 7, COL_B + 8
+AUTOAUGMENT_POLICIES = ("imagenet", "cifar10", "svhn")
+AA_NUM_BINS = 10                # AutoAugment's magnitude tables have 10 entries
 AUG_MAX_PIXELS = 65793          # kAugMaxPixels: 255 H W < 2^24, so Contrast's float32 mean is exact in torchvision's order
 NUM_BINS = 31
 ERASE_SCALE = (0.02, 0.33)
@@ -26,7 +34,8 @@ ERASE_RATIO = (0.3, 3.3)
 STREAM_ID = 0x61756721          # the fourth word of the draw stream's key: BatchMix keys its stream with three
 
 # the kernel's op codes (AugOp in csrc/augment.cu)
-K_IDENTITY, K_AFFINE, K_ROT90, K_BRIGHTNESS, K_COLOR, K_CONTRAST, K_SHARPNESS, K_POSTERIZE, K_SOLARIZE, K_AUTOCONTRAST, K_EQUALIZE = range(11)
+K_IDENTITY, K_AFFINE, K_ROT90, K_BRIGHTNESS, K_COLOR, K_CONTRAST, K_SHARPNESS, K_POSTERIZE, K_SOLARIZE, K_AUTOCONTRAST, K_EQUALIZE, \
+    K_INVERT = range(12)
 
 
 @functools.lru_cache(maxsize=None)
@@ -36,9 +45,38 @@ def _policy():
     return TrivialAugmentWide(num_magnitude_bins=NUM_BINS, interpolation=InterpolationMode.BILINEAR)
 
 
+@functools.lru_cache(maxsize=None)
+def _aa_policy(policy: str):
+    from torchvision.transforms import AutoAugmentPolicy, InterpolationMode
+    from torchvision.transforms.v2 import AutoAugment
+    return AutoAugment(AutoAugmentPolicy(policy), interpolation=InterpolationMode.BILINEAR)
+
+
 def op_names():
     """The 14 ops in the order of torchvision's ``TrivialAugmentWide._AUGMENTATION_SPACE``."""
     return tuple(_policy()._AUGMENTATION_SPACE.keys())
+
+
+def chain_names():
+    """The op index space of the tables' reference columns: :func:`op_names` and AutoAugment's ``Invert``."""
+    return op_names() + ("Invert",)
+
+
+def sub_policies(policy: str):
+    """AutoAugment's 25 sub-policies of ``policy``, ``((name, p, magnitude_idx), (name, p, magnitude_idx))``, as
+    torchvision's own ``AutoAugment`` object holds them."""
+    return tuple(_aa_policy(policy)._policies)
+
+
+def aa_magnitude(policy: str, name: str, magnitude_idx, negate: bool, H: int, W: int) -> float:
+    """The magnitude AutoAugment applies for an entry: ``_AUGMENTATION_SPACE[name][0](10, H, W)[magnitude_idx]``, negated
+    for a signed op when ``negate`` (0.0 for the ops without a table)."""
+    fn, signed = _aa_policy(policy)._AUGMENTATION_SPACE[name]
+    mags = fn(AA_NUM_BINS, H, W)
+    if mags is None:
+        return 0.0
+    m = float(mags[magnitude_idx])
+    return -m if (signed and negate) else m
 
 
 def magnitude(op: int, bin_: int, negate: bool, H: int, W: int) -> float:
@@ -71,9 +109,14 @@ def _grid_theta(matrix, H: int, W: int):
 @functools.lru_cache(maxsize=65536)
 def encode(op: int, bin_: int, negate: bool, H: int, W: int):
     """Kernel code and parameters (prm[0..6]) of one draw, with the scalars rounded as torchvision rounds them."""
-    from torchvision.transforms.v2.functional._geometry import _get_inverse_affine_matrix
     mag = magnitude(op, bin_, negate, H, W)          # raises for an op index or bin out of range
-    name = op_names()[op]
+    return op_code(op_names()[op], mag, H, W)
+
+
+def op_code(name: str, mag: float, H: int, W: int):
+    """Kernel code and parameters of op ``name`` at magnitude ``mag`` (as ``_apply_image_or_video_transform`` takes them)
+    on an ``H x W`` image, with the scalars rounded as torchvision rounds them."""
+    from torchvision.transforms.v2.functional._geometry import _get_inverse_affine_matrix
     if name in ("ShearX", "ShearY", "TranslateX", "TranslateY", "Rotate"):
         # the arguments _apply_image_or_video_transform gives F.affine / F.rotate, turned into affine_image's and
         # rotate_image's center_f, translate and shear
@@ -82,7 +125,7 @@ def encode(op: int, bin_: int, negate: bool, H: int, W: int):
             if angle == 0:
                 return (K_IDENTITY,)
             if angle == 180:
-                raise ValueError("Rotate by 180 is not in TrivialAugmentWide's range")
+                raise ValueError("Rotate by 180 is not in the range of TrivialAugmentWide or AutoAugment")
             if H == W and angle in (90, 270):
                 return (K_ROT90, 1 if angle == 90 else 3)
             matrix = _get_inverse_affine_matrix([0.0, 0.0], -angle, [0.0, 0.0], 1.0, [0.0, 0.0])
@@ -110,7 +153,35 @@ def encode(op: int, bin_: int, negate: bool, H: int, W: int):
         return (K_AUTOCONTRAST,)
     if name == "Equalize":
         return (K_EQUALIZE,)
+    if name == "Invert":
+        return (K_INVERT,)
     return (K_IDENTITY,)
+
+
+@functools.lru_cache(maxsize=64)
+def chain_table(policy: str, H: int, W: int) -> np.ndarray:
+    """Every outcome of one AutoAugment draw on an ``H x W`` image, encoded once: ``[25 * 16, AUG_CHAIN_PRM]`` float32, row
+    ``16 * sub_policy + 4 * applied + signs`` (bit 0 of ``applied`` / ``signs``: the first entry is applied / negated,
+    bit 1: the second).  A skipped entry is Identity; an applied first entry is op A, and a second entry applied alone is
+    op B after an Identity op A."""
+    names = chain_names()
+    subs = sub_policies(policy)
+    rows = np.zeros((len(subs) * 16, AUG_CHAIN_PRM), dtype=np.float32)
+    rows[:, 12] = rows[:, COL_B + 7] = names.index("Identity")
+    for i, sub in enumerate(subs):
+        for applied in range(4):
+            for signs in range(4):
+                r = rows[16 * i + 4 * applied + signs]
+                for k, (name, _, idx) in enumerate(sub):
+                    if not applied >> k & 1:
+                        continue
+                    mag = aa_magnitude(policy, name, idx, bool(signs >> k & 1), H, W)
+                    col = 0 if k == 0 else COL_B
+                    code = op_code(name, mag, H, W)
+                    r[col:col + len(code)] = code
+                    ref = 12 if k == 0 else COL_B + 7
+                    r[ref], r[ref + 1] = names.index(name), mag
+    return rows
 
 
 def erase_params(rng: np.random.Generator, H: int, W: int):
@@ -132,9 +203,11 @@ def erase_params(rng: np.random.Generator, H: int, W: int):
 
 
 class BatchAugment:
-    """The training-time input policy: per-sample TrivialAugment Wide and random erasing draws, and their application.
+    """The training-time input policy: per-sample TrivialAugment Wide or AutoAugment and random erasing draws, and their
+    application.
 
-    ``draw(n, H, W)`` runs on the host for every training batch and fills one of two pinned ``[n, AUG_PRM]`` tables (the
+    ``draw(n, H, W)`` runs on the host for every training batch and fills one of two pinned ``[n, width]`` tables
+    (``width``: ``AUG_CHAIN_PRM`` for an AutoAugment policy, ``AUG_PRM`` otherwise; the
     prefetcher copies a batch while it stages the next one, so a table is not rewritten while its copy may be in flight).
     The draws come from ``numpy.random.Generator(PCG64([seed, rank, epoch, STREAM_ID]))``: ``set_epoch`` re-keys the stream,
     so a resume at an epoch boundary replays the same draws.  Without a seed, the seed comes from OS entropy.
@@ -142,16 +215,18 @@ class BatchAugment:
 
     def __init__(self, auto_augment: Optional[str] = "ta_wide", random_erase: float = 0.0, seed: Optional[int] = None,
                  rank: int = 0):
-        if auto_augment not in (None, "ta_wide"):
-            raise ValueError("unknown auto-augment policy %r (only 'ta_wide')" % (auto_augment,))
+        if auto_augment not in (None, "ta_wide") + AUTOAUGMENT_POLICIES:
+            raise ValueError("unknown auto-augment policy %r (one of 'ta_wide', %s)"
+                             % (auto_augment, ", ".join(repr(p) for p in AUTOAUGMENT_POLICIES)))
         if not 0.0 <= random_erase <= 1.0:
             raise ValueError("random_erase must lie in [0, 1], got %r" % (random_erase,))
         self.auto_augment = auto_augment
+        self.width = AUG_CHAIN_PRM if auto_augment in AUTOAUGMENT_POLICIES else AUG_PRM
         self.random_erase = float(random_erase)
         self.seed = (int(seed) if seed is not None else np.random.SeedSequence().entropy) % (1 << 128)
         self.rank = int(rank)
         pin = torch.cuda.is_available()
-        self._slots = [torch.zeros((0, AUG_PRM), dtype=torch.float32) for _ in range(2)]
+        self._slots = [torch.zeros((0, self.width), dtype=torch.float32) for _ in range(2)]
         self._events = [None, None]
         self._pin = pin
         self._next = 0
@@ -172,10 +247,25 @@ class BatchAugment:
             self._events[k].synchronize()
             self._events[k] = None
         if self._slots[k].size(0) < n:
-            t = torch.zeros((n, AUG_PRM), dtype=torch.float32)
+            t = torch.zeros((n, self.width), dtype=torch.float32)
             self._slots[k] = t.pin_memory() if self._pin else t
         tab = self._slots[k][:n]
         rng = self.rng
+        if self.auto_augment in AUTOAUGMENT_POLICIES:
+            rows = self._draw_chain(rng, n, H, W)
+        else:
+            rows = self._draw_trivial(rng, n, H, W)
+        erase = rng.random(n) < self.random_erase if self.random_erase > 0 else np.zeros(n, dtype=bool)
+        for s in np.flatnonzero(erase):
+            box = erase_params(rng, H, W)
+            if box is not None:
+                rows[s, 7] = 1.0
+                rows[s, 8:12] = box
+        tab.copy_(torch.from_numpy(rows))
+        return tab
+
+    def _draw_trivial(self, rng, n: int, H: int, W: int) -> np.ndarray:
+        """TrivialAugment Wide (or, without a policy, Identity) rows: op, bin and sign per sample."""
         n_ops = len(op_names())
         if self.auto_augment is not None:
             ops = rng.integers(0, n_ops, n)
@@ -184,7 +274,6 @@ class BatchAugment:
         else:
             ops = bins = np.zeros(n, dtype=np.int64)
             neg = np.zeros(n, dtype=bool)
-        erase = rng.random(n) < self.random_erase if self.random_erase > 0 else np.zeros(n, dtype=bool)
         rows = np.zeros((n, AUG_PRM), dtype=np.float32)
         names = op_names()
         for s in range(n):
@@ -195,13 +284,18 @@ class BatchAugment:
                 rows[s, 13] = magnitude(int(ops[s]), int(bins[s]), bool(neg[s]), H, W)
             else:
                 rows[s, 12] = names.index("Identity")
-            if erase[s]:
-                box = erase_params(rng, H, W)
-                if box is not None:
-                    rows[s, 7] = 1.0
-                    rows[s, 8:12] = box
-        tab.copy_(torch.from_numpy(rows))
-        return tab
+        return rows
+
+    def _draw_chain(self, rng, n: int, H: int, W: int) -> np.ndarray:
+        """AutoAugment rows: a sub-policy uniformly, each entry applied iff ``u <= p``, a signed magnitude negated iff
+        ``v <= 0.5``; gathered from :func:`chain_table`."""
+        subs = sub_policies(self.auto_augment)
+        p = np.array([[e[1] for e in sub] for sub in subs], dtype=np.float64)
+        sub = rng.integers(0, len(subs), n)
+        applied = rng.random((n, 2)) <= p[sub]
+        neg = rng.random((n, 2)) <= 0.5
+        idx = 16 * sub + 4 * (applied[:, 0] + 2 * applied[:, 1]) + (neg[:, 0] + 2 * neg[:, 1])
+        return chain_table(self.auto_augment, H, W)[idx]
 
     def copied(self, table: torch.Tensor, event) -> None:
         """The consumer enqueued its copy of ``table`` (the last ``draw``); ``event`` completes when it is done."""
@@ -222,18 +316,21 @@ class BatchAugment:
     @staticmethod
     def reference_apply(src: torch.Tensor, prm: torch.Tensor, a: torch.Tensor, b: torch.Tensor, dtype: torch.dtype,
                         channels_last: bool) -> torch.Tensor:
-        """The CPU path: ``transforms.v2.functional`` per sample (through TrivialAugmentWide's own op dispatch), the
-        normalisation ``fp32(x * a[c] + b[c])`` rounded once, as the kernels' FMA, and the erase box set to 0."""
+        """The CPU path: ``transforms.v2.functional`` per sample (through torchvision's own op dispatch; op B of a two-op row
+        on op A's output), the normalisation ``fp32(x * a[c] + b[c])`` rounded once, as the kernels' FMA, and the erase box
+        set to 0."""
         pol = _policy()
-        names = op_names()
+        names = chain_names()
         p = prm.detach().cpu().numpy()
         a64 = a.detach().cpu().double().view(1, 3, 1, 1)
         b64 = b.detach().cpu().double().view(1, 3, 1, 1)
         src = src.cpu()
         out = []
         for s in range(src.size(0)):
-            img = pol._apply_image_or_video_transform(src[s], names[int(p[s, 12])], float(p[s, 13]), interpolation=pol.interpolation,
-                                                      fill=pol._fill)
+            img = src[s]
+            for col in ((12, COL_B + 7) if p.shape[1] == AUG_CHAIN_PRM else (12,)):
+                img = pol._apply_image_or_video_transform(img, names[int(p[s, col])], float(p[s, col + 1]),
+                                                          interpolation=pol.interpolation, fill=pol._fill)
             out.append(img)
         x = torch.stack(out).double()
         # x * a + b is exact in float64 (8-bit x times a 24-bit a, plus b, spans fewer than 53 bits): one rounding to fp32

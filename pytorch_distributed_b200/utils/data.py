@@ -121,15 +121,19 @@ def build_loaders(args, batch_size: int, distributed: bool = True, raw_uint8: bo
 
 
 def train_transforms(args, raw_uint8: bool = False):
-    """The ``ImageFolder`` training transforms: the crop and flip, then (``--auto-augment ta_wide``) TrivialAugmentWide on the
-    crop and (``--random-erase P``) RandomErasing after ``Normalize``, in the order of torchvision's classification recipe.
+    """The ``ImageFolder`` training transforms: the crop and flip, then (``--auto-augment ta_wide``) TrivialAugmentWide or
+    (``--auto-augment imagenet|cifar10|svhn``) AutoAugment on the crop and (``--random-erase P``) RandomErasing after
+    ``Normalize``, in the order of torchvision's classification recipe.
     With ``raw_uint8`` the workers ship uint8 tensors and the prefetcher normalises and augments them."""
     import torchvision.transforms as transforms
     t = [transforms.RandomResizedCrop(args.image_size), transforms.RandomHorizontalFlip()]
     if raw_uint8:
         return t + [transforms.PILToTensor()]
-    if getattr(args, "auto_augment", None) == "ta_wide":
+    policy = getattr(args, "auto_augment", None)
+    if policy == "ta_wide":
         t.append(transforms.TrivialAugmentWide(interpolation=transforms.InterpolationMode.BILINEAR))
+    elif policy is not None:
+        t.append(transforms.AutoAugment(transforms.AutoAugmentPolicy(policy), interpolation=transforms.InterpolationMode.BILINEAR))
     t += [transforms.ToTensor(), transforms.Normalize(mean=IMAGENET_MEAN, std=IMAGENET_STD)]
     p = float(getattr(args, "random_erase", 0.0) or 0.0)
     if p > 0:

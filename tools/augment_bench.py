@@ -1,13 +1,19 @@
 """Per-op time of ``augment_normalize`` (csrc/augment.cu) against ``normalize_nhwc`` at 256 x 3 x 224 x 224, bf16 channels_last,
 with bytes computed from the shapes and the share of 3.35 TB/s (H100 SXM HBM3); for context, torchvision v2 run per sample on
-CUDA tensors.  Prints one JSON line per row.
+CUDA tensors.  Prints one JSON line per row, each with the card's name, power limit and SM clock.
+
+AutoAugment rows (two launches through a uint8 scratch batch): one per ImageNet sub-policy with both ops forced on, one
+per policy for a drawn batch, and the host ``draw()`` time of each policy.  The bytes are the same read-once-write-once
+bound; the scratch batch's write and read are not counted.
 
     python tools/augment_bench.py [--batch 256] [--size 224] [--iters 50] [--tv-samples 64]
 """
 import argparse
 import json
 import os
+import subprocess
 import sys
+import time
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
@@ -71,10 +77,52 @@ def main():
     ms = _time(lambda: [tf(src[s]) for s in range(k)], max(3, a.iters // 10)) * n / k
     rows.append({"op": "torchvision_v2_per_sample", "ms": ms, "bytes": moved, "GBps": moved / (ms * 1e-3) / 1e9,
                  "share_of_3.35TBps": moved / PEAK / (ms * 1e-3), "bound": "launch/host"})
-    name = torch.cuda.get_device_name()
+    rows += autoaugment_rows(C, A, src, ca, cb, n, H, a.iters, moved)
+    card = device_info()
     for r in rows:
-        r.update(device=name, batch=n, size=H)
+        r.update(card, batch=n, size=H)
+        if "ms" in r:
+            r["us"] = r["ms"] * 1e3
+            r["TBps"] = r["bytes"] / (r["ms"] * 1e-3) / 1e12
         print(json.dumps(r))
+
+
+def device_info():
+    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.sm", "--format=csv,noheader",
+                        "-i", str(torch.cuda.current_device())], capture_output=True, text=True)
+    name, power, clock = ([v.strip() for v in q.stdout.split(",")] + ["?"] * 3)[:3] if q.returncode == 0 else ["?"] * 3
+    return {"device": torch.cuda.get_device_name(), "power_limit": power, "sm_clock": clock, "nvidia_smi_name": name}
+
+
+def autoaugment_rows(C, A, src, ca, cb, n, H, iters, moved):
+    rows = []
+    table = torch.from_numpy(A.chain_table("imagenet", H, H))
+    for i, sub in enumerate(A.sub_policies("imagenet")):
+        idx = torch.tensor([16 * i + 12 + (s & 3) for s in range(n)])    # both entries applied, the four sign patterns
+        prm = table[idx].clone()
+        prm[:, 7] = 1.0
+        prm[:, 8:12] = torch.tensor([50, 60, 40, 30])
+        prm = prm.cuda()
+        ms = _time(lambda: C.augment_normalize(src, prm, ca, cb, 1, True), iters)
+        rows.append({"op": "imagenet[%d] %s+%s" % (i, sub[0][0], sub[1][0]), "ms": ms, "bytes": moved})
+    for policy in A.AUTOAUGMENT_POLICIES:
+        aug = A.BatchAugment(policy, 0.1, seed=0)
+        prm = aug.draw(n, H, H).cuda()
+        ms = _time(lambda: C.augment_normalize(src, prm, ca, cb, 1, True), iters)
+        rows.append({"op": "drawn batch: %s" % policy, "ms": ms, "bytes": moved})
+    for policy in ("ta_wide",) + A.AUTOAUGMENT_POLICIES:
+        aug = A.BatchAugment(policy, 0.1, seed=0)
+        aug.draw(n, H, H)
+        t0 = time.perf_counter()
+        for _ in range(20):
+            aug.draw(n, H, H)
+        rows.append({"op": "host draw(): %s" % policy, "host_ms": (time.perf_counter() - t0) / 20 * 1e3})
+    for r in rows:
+        if "ms" in r:
+            r["GBps"] = r["bytes"] / (r["ms"] * 1e-3) / 1e9
+            r["share_of_3.35TBps"] = r["bytes"] / PEAK / (r["ms"] * 1e-3)
+            r["bound"] = "memory"
+    return rows
 
 
 if __name__ == "__main__":
